@@ -384,7 +384,7 @@ constexpr uint32_t kFootCap = 1024;  // footers buffered per segment (ring offse
 
 struct SendPlanState {  // producer-only
   uint64_t rt, cap, staging, total_left, written_total, ncalls, cur, bidx, last_rh;
-  uint32_t partial, max_sge;
+  uint32_t partial, max_sge, coalesce;
 };
 
 struct SendCallScratch {  // frames of the call being published
@@ -541,6 +541,130 @@ __device__ __noinline__ void send_produce_segment(const SendOpDev& op, const Pai
   __syncwarp();
 }
 
+// Producer, coalesced framing (B200_SEND_COALESCE, DESIGN.md §2): every Send call writes ONE frame that
+// gathers the bytes of the slices [cur, cur + kCoalesceSlices) from byte `bidx` on, p = min(those bytes,
+// CWS(staging), CWS(free)).  Two walks over the window, 32 slices at a time with a running prefix: the
+// first finds p, the second publishes each slice's part of the frame at payload offset `prefix` and finds
+// where the cursor stops.  Slices share 8-byte words of the frame, so nothing here writes whole words
+// of payload: short parts are stored byte by byte by the planner lane, longer ones go to the movers,
+// whose stores are byte-exact at the edges of an item.
+__device__ __noinline__ void send_produce_coalesced(const SendOpDev& op, const PairDev* P, uint8_t* ring,
+                                                    SendPlanState& S, SendCallScratch& CS, WorkItem* q, PipeCtl* ctl,
+                                                    uint32_t* foot8, uint32_t* nfoot_out, uint32_t lane) {
+  const uint64_t cap = S.cap, mask = cap - 1;
+  uint32_t base_item = 0, nfoot = 0;
+  bool op_done = false;
+  while (nfoot < kFootCap) {
+    const uint64_t rt = S.rt;
+    const uint64_t rh = ld_volatile_u64(&P->credit_head);  // credit snapshot, once per call (see above)
+    if (rh != S.last_rh) {
+      if (P->wire != 0) __threadfence_system();
+      else __threadfence();
+      S.last_rh = rh;
+    }
+    const uint64_t cur = S.cur, bidx = S.bidx;
+    const uint64_t wend = op.nreal < cur + kCoalesceSlices ? op.nreal : cur + kCoalesceSlices;
+    const uint64_t ws = calc_writable(S.staging), wf = calc_writable(free_size(cap, rh, rt));
+    const uint64_t pmax = ws < wf ? ws : wf;
+    uint64_t p = 0;
+    for (uint64_t g = cur; g < wend && p < pmax; g += 32) {
+      const uint64_t idx = g + lane;
+      uint64_t len = idx < wend ? op.slices[idx].len - (idx == cur ? bidx : 0) : 0;
+      for (int o = 16; o > 0; o >>= 1) len += __shfl_xor_sync(0xffffffffu, len, o);
+      p += len;
+    }
+    if (p > pmax) p = pmax;
+    uint64_t pre = 0, passed = 0, nb = 0;
+    bool cut = false;
+    for (uint64_t g = cur; g < wend && pre < p; g += 32) {
+      const uint64_t idx = g + lane;
+      const bool valid = idx < wend;
+      const uint8_t* ptr = nullptr;
+      uint64_t len = 0, skip = 0;
+      if (valid) {
+        const SliceDev sl = op.slices[idx];
+        skip = idx == cur ? bidx : 0;
+        ptr = sl.ptr + skip;
+        len = sl.len - skip;
+      }
+      uint64_t incl = len;
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint64_t t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= (uint32_t)o) incl += t;
+      }
+      const uint64_t a = pre + incl - len, e = pre + incl;  // this slice's bytes are frame payload [a, e)
+      const uint64_t n = valid && a < p ? (e < p ? e : p) - a : 0;
+      // cursor advance (rdma_flush, rdma_bp_posix.cc:480-493): a slice is passed when the bytes reach
+      // past its end (zero-length slices too, unless the call ended right before them); the first slice
+      // the bytes end inside stays current
+      passed += __popc(__ballot_sync(0xffffffffu, valid && a < p && e <= p));
+      const unsigned cm = __ballot_sync(0xffffffffu, valid && a < p && e > p);
+      if (cm) {
+        nb = __shfl_sync(0xffffffffu, skip + (p - a), __ffs(cm) - 1);
+        cut = true;
+      }
+      const bool tiny = n != 0 && n <= kTiny;
+      const uint32_t items = (n && !tiny) ? (uint32_t)((n + kChunk - 1) / kChunk) : 0;
+      uint32_t items_incl = items;
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, items_incl, o);
+        if (lane >= (uint32_t)o) items_incl += t;
+      }
+      const uint32_t nitems = __shfl_sync(0xffffffffu, items_incl, 31);
+      const uint64_t foff = (rt + 8 + a) & mask;
+      if (tiny) {
+#pragma unroll 1
+        for (uint32_t i = 0; i < (uint32_t)n; i++) ring[(foff + i) & mask] = __ldg(ptr + i);
+      }
+      CS.first_item[lane] = items_incl - items;
+      CS.src[lane] = ptr;
+      CS.len[lane] = n;
+      CS.off[lane] = foff;
+      __syncwarp();
+      // items in id order, 32 at a time; item `it` belongs to the last slice whose first item is <= it
+      for (uint32_t it = lane; it < nitems; it += 32) {
+        uint32_t f = 0;
+        while (f + 1 < 32 && CS.first_item[f + 1] <= it) f++;
+        const uint64_t c0 = (uint64_t)(it - CS.first_item[f]) * kChunk;
+        uint64_t m = CS.len[f] - c0;
+        if (m > kChunk) m = kChunk;
+        publish_item(q, base_item + it, reinterpret_cast<uint64_t>(CS.src[f] + c0), (CS.off[f] + c0) & mask, 0,
+                     (uint32_t)m);
+      }
+      __syncwarp();
+      base_item += nitems;
+      pre = __shfl_sync(0xffffffffu, e, 31);
+    }
+    if (lane == 0) {
+      if (p) {
+        *reinterpret_cast<uint64_t*>(ring + rt) = p;  // AppendHeader
+        foot8[nfoot] = (uint32_t)(((rt + 8 + round_up8(p)) & mask) >> 3);
+        S.rt = (rt + encoded_size(p)) & mask;
+        S.ncalls++;
+        S.cur = cur + passed;
+        S.bidx = cut ? nb : 0;
+      }
+      S.partial = p < S.total_left;  // pair.cc:712
+      S.total_left -= p;
+      S.written_total += p;
+    }
+    __syncwarp();
+    if (p) nfoot++;
+    if (p == 0 || !(op.flags & kFlagUntilBlocked) || S.total_left == 0) {
+      op_done = true;
+      break;
+    }
+  }
+  if (lane == 0) {
+    *nfoot_out = nfoot;
+    ctl->total_items = base_item;
+    ctl->op_done = op_done ? 1u : 0u;
+    __threadfence_block();
+    *(volatile uint32_t*)&ctl->seg_done = 1;
+  }
+  __syncwarp();
+}
+
 // Send mover: source = a slice at any alignment (linear), destination = the peer ring (may wrap).
 struct SendMove {
   uint8_t* ring;
@@ -592,7 +716,9 @@ __device__ __forceinline__ void send_body(PairDev* __restrict__ pairs, const Sen
     PS.rt = *(volatile uint64_t*)&P->remote_tail;
     PS.cap = *(volatile uint64_t*)&P->cap;
     PS.staging = PS.cap / 2;  // send_buf_size = recv_buf_size / 2, pair.cc:104
-    PS.max_sge = *(volatile uint32_t*)&P->max_sge;
+    const uint32_t sge = *(volatile uint32_t*)&P->max_sge;
+    PS.max_sge = sge & ~kSgeCoalesce;
+    PS.coalesce = (sge & kSgeCoalesce) != 0;
     PS.cur = 0;
     PS.bidx = op.byte_idx;
     PS.written_total = 0;
@@ -630,7 +756,8 @@ __device__ __forceinline__ void send_body(PairDev* __restrict__ pairs, const Sen
     }
     __syncthreads();
     if (warp == 0) {
-      send_produce_segment(op, P, ring, PS, CS, q, &ctl, foot8, &s_nfoot, lane);
+      if (PS.coalesce) send_produce_coalesced(op, P, ring, PS, CS, q, &ctl, foot8, &s_nfoot, lane);
+      else send_produce_segment(op, P, ring, PS, CS, q, &ctl, foot8, &s_nfoot, lane);
     } else {  // ---------------------------------------------- move bytes
       const SendMove mv{ring, cap, mask};
       mover_run(mv, q, &ctl, stage_mem + (warp - 1) * (kDepth * kStageBytes), &bars[(warp - 1) * kDepth], phase_bits, lane);
@@ -1564,6 +1691,119 @@ __device__ __forceinline__ void svc_send_small(const SvcParams& sp, const ConnVi
   __syncwarp();
 }
 
+// ---- one coalesced Send call by one warp (B200_SEND_COALESCE, DESIGN.md §2): <= kSvcInline slices, <= kSmallMax
+// bytes, ONE frame of p = min(bytes from byte_idx, CWS(staging), CWS(free)).  The slices sit at any offset of
+// the frame, so every lane assembles whole payload words itself (word j = frame bytes [8 j, 8 j + 8), gathered
+// from the one or more slices it covers) and no two lanes store to the same word.  The eager push to the peer's
+// host slot works as for a per-slice first frame.
+__device__ __forceinline__ uint8_t ld_sys_u8(const void* p) {
+  uint16_t v;
+  asm volatile("ld.relaxed.sys.global.u8 %0, [%1];" : "=h"(v) : "l"(p) : "memory");
+  return (uint8_t)v;
+}
+__device__ __forceinline__ void svc_send_small_coalesced(const SvcParams& sp, const ConnView& cv, const SvcCmd& c,
+                                                         int pslot, OpResult& res, uint32_t lane) {
+  res.bytes = 0;
+  res.calls = 0;
+  PairDev& P = *cv.P;
+  if (P.status != kStConnected) return;  // pair.cc:657
+  const uint64_t cap = P.cap, mask = cap - 1;
+  uint8_t* ring = P.peer_ring;
+  const bool sys_scope = P.wire != 0;
+  const uint64_t rt = P.remote_tail;
+  const uint64_t rh = P.credit_head;  // credit snapshot, once
+  const int peer_slot = cv.Q ? P.peer_slot : -1;
+  if (sys_scope) __threadfence_system();
+  const uint32_t nsl = (uint32_t)c.n;
+  const uint32_t look = c.nreal;  // <= kSvcInline here, so within the kCoalesceSlices window
+  uint64_t raw = 0, len = 0;
+  const uint8_t* ptr = nullptr;
+  if (lane < nsl) {
+    raw = c.inl[lane].len;
+    if (lane < look) {
+      const uint64_t skip = lane == 0 ? c.byte_idx : 0;
+      ptr = c.inl[lane].ptr + skip;
+      len = raw - skip;
+    }
+  }
+  uint64_t total = raw;  // total_slice_size
+  for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+  total -= c.byte_idx;
+  uint64_t incl = len;
+  for (int o = 1; o < 8; o <<= 1) {
+    const uint64_t t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= (uint32_t)o) incl += t;
+  }
+  const uint64_t ws = calc_writable(cap / 2), wf = calc_writable(free_size(cap, rh, rt));
+  const uint64_t pmax = ws < wf ? ws : wf;
+  uint64_t p = __shfl_sync(0xffffffffu, incl, 7);
+  if (p > pmax) p = pmax;
+  const bool at_head = peer_slot >= 0 && p > 0 && cv.Q->remain == 0 && cv.Q->head == rt;
+  const bool eager = at_head && p <= kEagerMax && sp.erec != nullptr && cv.SQ->pushed_at != cv.SQ->delivered;
+  uint8_t* eslot = eager ? sp.eslots + (size_t)peer_slot * kEagerMax : nullptr;
+  uint64_t cs = 0;
+  const uint64_t a_mine = incl - len;  // frame payload offset of this lane's slice
+  const uint32_t words = (uint32_t)((p + 7) >> 3);
+  for (uint32_t base = 0; base < words; base += 32) {
+    const uint32_t j = base + lane;
+    const uint64_t b0 = 8ull * j, b1 = b0 + 8 < p ? b0 + 8 : p;
+    uint64_t w = 0;
+    for (int k = 0; k < (int)kSvcInline; k++) {  // the slices' (offset, length, source) from their lanes
+      const uint64_t ak = __shfl_sync(0xffffffffu, a_mine, k), lk = __shfl_sync(0xffffffffu, len, k);
+      const uint8_t* sk = reinterpret_cast<const uint8_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<uint64_t>(ptr), k));
+      const uint64_t s = ak > b0 ? ak : b0, e = ak + lk < b1 ? ak + lk : b1;
+      if (j >= words || s >= e) continue;
+      const uint8_t* src = sk + (s - ak);
+      if (e - s == 8) {  // the whole word from one slice: two aligned loads at most
+        const uintptr_t sa = reinterpret_cast<uintptr_t>(src);
+        const uint32_t sh = (uint32_t)(sa & 7) * 8;
+        const uint64_t* s0 = reinterpret_cast<const uint64_t*>(sa & ~(uintptr_t)7);
+        w = sh ? (ld_sys_u64(s0) >> sh) | (ld_sys_u64(s0 + 1) << (64 - sh)) : ld_sys_u64(s0);
+      } else {
+#pragma unroll 1
+        for (uint64_t i = s; i < e; i++) w |= (uint64_t)ld_sys_u8(src + (i - s)) << (8 * (i - b0));
+      }
+    }
+    if (j < words) {
+      *reinterpret_cast<uint64_t*>(ring + ((rt + 8 + b0) & mask)) = w;  // bytes past p are zero (pad)
+      if (eslot) {
+        st_sys_u64(eslot + b0, w);
+        cs ^= eager_word(w, j);
+      }
+    }
+  }
+  if (lane == 0 && p) *reinterpret_cast<uint64_t*>(ring + rt) = p;  // AppendHeader
+  if (sys_scope) __threadfence_system();  // footer last (see svc_send_small)
+  __syncwarp();
+  const uint64_t esum = p ? encoded_size(p) : 0;
+  if (lane == 0) {
+    if (p) *reinterpret_cast<uint64_t*>(ring + ((rt + 8 + round_up8(p)) & mask)) = kFooter;
+    PairDev* Pg = &sp.pairs[pslot];
+    P.remote_tail = (rt + esum) & mask;
+    P.partial_write = p < total;
+    VL(Pg->remote_tail) = (rt + esum) & mask;
+    VL(Pg->partial_write) = p < total;  // pair.cc:712
+    if (P.mirror) {
+      volatile PairMirror* vm = P.mirror;
+      vm->remote_tail = (rt + esum) & mask;
+      vm->partial_write = p < total;
+      vm->credit_head = rh;
+      vm->peer_exit = P.credit_exit;
+    }
+  }
+  res.bytes = p;
+  res.calls = p ? 1 : 0;
+  if (at_head) {
+    if (eager) eager_publish(sp, peer_slot, cv.SQ, cv.SQ->delivered, p, cs, lane);
+    if (lane == 0 && cv.Q->mirror) {
+      volatile PairMirror* vm = cv.Q->mirror;
+      vm->readable = p;
+      vm->has_message = 1;
+    }
+  }
+  __syncwarp();
+}
+
 // ---- one PairPollable::Recv call by one warp (ring_buffer.cc:122-191 + pair.cc:264-286).  Returns false
 // when the call would move more than kSmallMax bytes (nothing touched: the pool takes it).  With `discard`
 // the payload is not stored anywhere (Retire: the host already took it from the eager slot, the frame is the
@@ -1769,7 +2009,8 @@ __global__ void __launch_bounds__(128) k_svc_owner(SvcParams sp) {
         }
         if (small) {
           if (opc == kSvcSend) {
-            svc_send_small(sp, cv, c, pslot, res, lane);
+            if (cv.P->max_sge & kSgeCoalesce) svc_send_small_coalesced(sp, cv, c, pslot, res, lane);
+            else svc_send_small(sp, cv, c, pslot, res, lane);
             done_small = true;
             TRACE_MARK(0, tr0);  // small send: fetched -> frames landed, eager record + mirror stores issued
             if (owed) {

@@ -63,6 +63,7 @@ struct Config {
   int busy_poll_us = 500;                // GRPC_RDMA_BUSY_POLLING_TIMEOUT_US, config.cc:75-81
   int poller_sleep_ms = 1000;            // GRPC_RDMA_POLLER_SLEEP_TIMEOUT_MS, config.cc:83-89
   int max_sge = 30;                      // ibv_device_attr.max_sge on the authors' HCA
+  int send_coalesce = 0;                 // B200_SEND_COALESCE: one frame per Send call (DESIGN.md §2)
 };
 
 // Address blob: same 48-byte layout as grpc_core::ibverbs::Address::addr_
@@ -100,6 +101,7 @@ struct b200_pair {
   std::atomic<bool> peer_dead{false};  // ... and found gone (kept on the host: the mirror is re-published from the device)
   std::chrono::steady_clock::time_point last_probe{};
   int max_sge = 30;  // captured at Init (what the kernels use for this pair)
+  bool coalesce = false;  // B200_SEND_COALESCE, captured at Init like max_sge
   // service: payload bytes Recv has returned since the service started (the device keeps the same count;
   // an eagerly pushed frame is valid only while both agree), and the asynchronous Retire of the last
   // eagerly received frame, if it has not been confirmed yet
@@ -206,7 +208,7 @@ struct Runtime {
   SvcCmd* svc_cmds = nullptr;          // pinned, mapped  [nowners][kOwnQ]
   SvcDone* svc_done = nullptr;         // pinned, mapped  [nowners][kOwnQ]
   std::atomic<uint32_t>* svc_consumed = nullptr;  // host only [nowners][kOwnQ]: stamp of the last answer its waiter has read
-  SliceDev* svc_slices = nullptr;      // pinned, mapped  [nowners][kOwnQ][kSvcSliceArea]
+  SliceDev* svc_slices = nullptr;      // pinned, mapped  [nowners][kOwnQ][kSvcSliceArea + 1]
   EagerRec* svc_erec = nullptr;        // pinned, mapped  [kMaxPairs]
   uint8_t* svc_eslots = nullptr;       // pinned, mapped  [kMaxPairs][kEagerMax]
   BigBox* d_svc_boxes = nullptr;
@@ -408,6 +410,7 @@ static int init_locked(int device) {
   r.cfg.poller_sleep_ms = (int)env_long("GRPC_RDMA_POLLER_SLEEP_TIMEOUT_MS", 1000);
   r.cfg.max_sge = (int)env_long("GRPC_RDMA_MAX_SGE", 30);
   if (r.cfg.max_sge < 1 || r.cfg.max_sge > kMaxSgeLimit) r.cfg.max_sge = 30;
+  r.cfg.send_coalesce = env_long("B200_SEND_COALESCE", 0) == 1 ? 1 : 0;
 
   if (!CU_OK(cudaStreamCreateWithFlags(&r.stream, cudaStreamNonBlocking))) return -1;
   if (!CU_OK(cudaStreamCreateWithFlags(&r.poll_stream, cudaStreamNonBlocking))) return -1;
@@ -427,7 +430,7 @@ static int init_locked(int device) {
     return CU_OK(cudaHostAlloc(p, n, cudaHostAllocMapped | cudaHostAllocPortable));
   };
   if (!halloc((void**)&r.h_sop, sizeof(SendOpDev)) || !halloc((void**)&r.h_rop, sizeof(RecvOpDev)) ||
-      !halloc((void**)&r.h_slices, sizeof(SliceDev) * (kMaxSgeLimit + 1)) ||
+      !halloc((void**)&r.h_slices, sizeof(SliceDev) * (kCoalesceSlices + 1)) ||
       !halloc((void**)&r.h_res, sizeof(OpResult)) ||
       !halloc((void**)&r.h_scan_slots, sizeof(int32_t) * kMaxPairs) ||
       !halloc((void**)&r.h_scan_events, sizeof(uint32_t) * kMaxPairs) ||
@@ -535,6 +538,9 @@ extern "C" int b200_config_set(const char* key, const char* value) {
   } else if (k == "GRPC_RDMA_MAX_SGE") {
     if (v < 1 || v > kMaxSgeLimit) return -1;
     r.cfg.max_sge = (int)v;
+  } else if (k == "B200_SEND_COALESCE") {
+    if (v != 0 && v != 1) return -1;
+    r.cfg.send_coalesce = (int)v;
   } else {
     set_err("b200_config_set: unknown key " + k);
     return -1;
@@ -552,6 +558,7 @@ extern "C" int64_t b200_config_get(const char* key) {
   if (k == "GRPC_RDMA_BUSY_POLLING_TIMEOUT_US") return r.cfg.busy_poll_us;
   if (k == "GRPC_RDMA_POLLER_SLEEP_TIMEOUT_MS") return r.cfg.poller_sleep_ms;
   if (k == "GRPC_RDMA_MAX_SGE") return r.cfg.max_sge;
+  if (k == "B200_SEND_COALESCE") return r.cfg.send_coalesce;
   return -1;
 }
 
@@ -648,6 +655,9 @@ extern "C" b200_pair* b200_pool_get(const char* id) {
   return it == r.id_pair.end() ? nullptr : it->second;
 }
 
+// the pair's max_sge word of PairDev: the mode rides in its top bit so the line stays 128 bytes
+static uint32_t sge_word(const b200_pair* p) { return (uint32_t)p->max_sge | (p->coalesce ? kSgeCoalesce : 0u); }
+
 extern "C" void b200_pair_init(b200_pair* p) {
   if (!p || !ensure_init()) return;
   Runtime& r = R();
@@ -680,9 +690,10 @@ extern "C" void b200_pair_init(b200_pair* p) {
   hd.cap = cap;
   hd.mirror = p->mirror;
   hd.status = B200_INITIALIZED;
-  hd.max_sge = (uint32_t)r.cfg.max_sge;
-  hd.peer_slot = -1;
   p->max_sge = r.cfg.max_sge;
+  p->coalesce = r.cfg.send_coalesce != 0;
+  hd.max_sge = sge_word(p);
+  hd.peer_slot = -1;
   p->svc_delivered = 0;
   p->retire_pending = false;
   p->peer_dead = false;
@@ -818,7 +829,7 @@ extern "C" int b200_pair_connect(b200_pair* p, const void* peer48, size_t n) {
     hd.mirror = p->mirror;
     hd.peer_mirror = nullptr;
     hd.status = B200_CONNECTED;
-    hd.max_sge = (uint32_t)p->max_sge;
+    hd.max_sge = sge_word(p);
     hd.peer_slot = -1;
     hd.wire = 1;  // system-scope fences: the ring is in another GPU's HBM, reached over NVLink
     if (!write_setup(r, p, hd)) {
@@ -857,7 +868,7 @@ extern "C" int b200_pair_connect(b200_pair* p, const void* peer48, size_t n) {
   hd.mirror = p->mirror;
   hd.peer_mirror = q->mirror;
   hd.status = B200_CONNECTED;
-  hd.max_sge = (uint32_t)p->max_sge;
+  hd.max_sge = sge_word(p);
   hd.peer_slot = q->slot;
   hd.wire = 0;
   if (!write_setup(r, p, hd)) {
@@ -1045,7 +1056,7 @@ extern "C" int b200_service_start(int workers) {
     if (!*st && !CU_OK(cudaStreamCreateWithFlags(st, cudaStreamNonBlocking))) return -1;
   const size_t nent = (size_t)owners * kOwnQ;
   if (!halloc((void**)&r.svc_cmds, sizeof(SvcCmd) * nent) || !halloc((void**)&r.svc_done, sizeof(SvcDone) * nent) ||
-      !halloc((void**)&r.svc_slices, sizeof(SliceDev) * nent * kSvcSliceArea) ||
+      !halloc((void**)&r.svc_slices, sizeof(SliceDev) * nent * (kSvcSliceArea + 1)) ||
       !halloc((void**)&r.svc_erec, sizeof(EagerRec) * kMaxPairs) ||
       !halloc((void**)&r.svc_eslots, (size_t)kEagerMax * kMaxPairs) ||
       !halloc((void**)&r.svc_ready, sizeof(ReadyEntry) * kReadyRing) || !halloc((void**)&r.svc_host_scans, 64))
@@ -1118,7 +1129,7 @@ static bool svc_try_post(Runtime& r, int q, Fill fill, uint64_t* ticket) {
   Q.next = t + 1;
   SvcCmd* c = &r.svc_cmds[e];
   c->nreal = 0;
-  fill(c, r.svc_slices + e * kSvcSliceArea);
+  fill(c, r.svc_slices + e * (kSvcSliceArea + 1));
   c->op = (c->op & 0xffu) | ((r.svc_gen.load(std::memory_order_acquire) & 0xffffffu) << 8);
   std::atomic_thread_fence(std::memory_order_release);
   *(volatile uint32_t*)&c->stamp2 = (uint32_t)(t + 1);
@@ -1278,9 +1289,13 @@ static bool svc_fill_send(b200_pair* p, SvcCmd* c, SliceDev* area, const b200_sl
                           uint32_t flags, uint64_t* bounce_cursor = nullptr, uint8_t* own_bounce = nullptr,
                           uint64_t own_bounce_cap = 0) {
   const bool one_call = !(flags & B200_BATCH_UNTIL_BLOCKED);  // (flags >> 16: owed Retire)
+  const size_t window = p->coalesce ? kCoalesceSlices : (size_t)p->max_sge;
   size_t look = n;
-  if (one_call && look > (size_t)p->max_sge) look = (size_t)p->max_sge;
-  if (look > kSvcSliceArea - 1) look = kSvcSliceArea - 1;
+  if (one_call && look > window) look = window;  // coalesced: up to kSvcSliceArea, the pseudo-slice goes behind
+  if (!one_call && look > kSvcSliceArea - 1) look = kSvcSliceArea - 1;
+  // coalesced: ONE frame of at most CWS(C/2) bytes gathers all of them, so the call stages at most C/2 in all
+  const bool coal = one_call && p->coalesce;
+  uint64_t budget = p->cap / 2;
   TlsBounce own;  // an op that outlives the call brings its own staging
   own.tx = own_bounce;
   own.tx_cap = own_bounce_cap;
@@ -1296,9 +1311,15 @@ static bool svc_fill_send(b200_pair* p, SvcCmd* c, SliceDev* area, const b200_sl
     const uint64_t skip = i == 0 ? byte_idx : 0;
     uint64_t take = len - skip;
     if (one_call && take > p->cap / 2) take = p->cap / 2;  // a call never accepts more than the staging size
+    if (coal) {
+      if (take > budget) take = budget;
+      budget -= take;
+    }
     if (bounce_off + take > tb.tx_cap) {
-      if (bounce_cursor == nullptr && bounce_off == 0) {
-        if (!ensure_bounce(&tb.tx, &tb.tx_cap, (one_call ? p->cap : take) + 16 * (kMaxSgeLimit + 4))) return false;
+      // (one call: the buffer is sized for everything the call can read, whichever slice first overflows it)
+      if (bounce_cursor == nullptr && (bounce_off == 0 || one_call)) {
+        const size_t slack = 16 * ((look > (size_t)kMaxSgeLimit ? look : (size_t)kMaxSgeLimit) + 4);
+        if (!ensure_bounce(&tb.tx, &tb.tx_cap, (one_call ? p->cap : take) + slack)) return false;
       } else if (!one_call) {
         look = i;  // staged prefix only; the rest only counts towards total_slice_size
         break;
@@ -1307,6 +1328,7 @@ static bool svc_fill_send(b200_pair* p, SvcCmd* c, SliceDev* area, const b200_sl
     bounce_off += (take + 15) & ~15ull;
   }
   bounce_off = bounce_cursor ? *bounce_cursor : 0;
+  budget = p->cap / 2;
   uint64_t rest = 0;
   for (size_t i = look; i < n; i++) rest += slices[i].len;
   const size_t nsl = look + (rest ? 1 : 0);
@@ -1318,6 +1340,10 @@ static bool svc_fill_send(b200_pair* p, SvcCmd* c, SliceDev* area, const b200_sl
       const uint64_t skip = i == 0 ? byte_idx : 0;
       uint64_t take = len - skip;
       if (one_call && take > p->cap / 2) take = p->cap / 2;
+      if (coal) {
+        if (take > budget) take = budget;
+        budget -= take;
+      }
       if (bounce_off + take > tb.tx_cap) take = tb.tx_cap - bounce_off;
       memcpy(tb.tx + bounce_off, ptr + skip, take);
       out[i].ptr = tb.tx + bounce_off - skip;  // keep (ptr + skip) pointing at the staged bytes
@@ -1474,11 +1500,13 @@ extern "C" uint64_t b200_pair_send(b200_pair* p, const b200_slice* slices, size_
   cudaSetDevice(r.dev);
   // One Send call looks at <= max_sge slices; the rest only contributes to
   // total_slice_size (pair.cc:661-664), folded into one trailing pseudo-slice
-  // that is never dereferenced.
-  const size_t look = n < (size_t)p->max_sge ? n : (size_t)p->max_sge;
+  // that is never dereferenced.  A coalesced call looks at <= kCoalesceSlices slices and, being one frame
+  // of at most CWS(C/2) bytes, reads at most C/2 bytes of all of them together.
+  const size_t window = p->coalesce ? kCoalesceSlices : (size_t)p->max_sge;
+  const size_t look = n < window ? n : window;
   uint64_t rest = 0;
   for (size_t i = look; i < n; i++) rest += slices[i].len;
-  uint64_t bounce_off = 0;
+  uint64_t bounce_off = 0, budget = p->cap / 2;
   for (size_t i = 0; i < look; i++) {
     const uint8_t* ptr = (const uint8_t*)slices[i].ptr;
     uint64_t len = slices[i].len;
@@ -1486,9 +1514,11 @@ extern "C" uint64_t b200_pair_send(b200_pair* p, const b200_slice* slices, size_
       // unregistered host memory: stage like the reference's send buffer
       const uint64_t skip = i == 0 ? byte_idx : 0;
       const uint64_t useful = len - skip;
-      const uint64_t limit = p->cap / 2;  // a call never accepts more than the staging size
+      const uint64_t limit = p->coalesce ? budget : p->cap / 2;  // a call never accepts more than the staging size
       uint64_t take = useful < limit ? useful : limit;
-      if (!ensure_bounce(&r.bounce_tx, &r.bounce_tx_cap, p->cap + 16 * (kMaxSgeLimit + 4))) return 0;
+      if (p->coalesce) budget -= take;
+      const uint64_t slack = 16 * ((p->coalesce ? kCoalesceSlices : kMaxSgeLimit) + 4);
+      if (!ensure_bounce(&r.bounce_tx, &r.bounce_tx_cap, p->cap + slack)) return 0;
       if (bounce_off + take > r.bounce_tx_cap) take = r.bounce_tx_cap - bounce_off;
       memcpy(r.bounce_tx + bounce_off, ptr + skip, take);
       // keep (ptr + skip) pointing at the staged bytes
