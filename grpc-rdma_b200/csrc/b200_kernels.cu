@@ -17,8 +17,8 @@
 // publishes 4 KiB work items; the mover warps pull every item's source bytes
 // into shared memory with the bulk-copy engine (cp.async.bulk + mbarrier
 // complete_tx, several stages in flight per warp, so the HBM read latency is
-// never held in registers) and write them out with aligned 16-byte vector
-// stores, re-aligning through a funnel shift when source and destination
+// never held in registers) and write them out with bulk stores, re-aligning
+// the stage in place through a funnel shift when source and destination
 // differ mod 16 (gRPC slices sit at odd offsets, ring payloads at 8 mod 16).
 // Byte granularity only at the <16-byte edges of a copy.
 #include <cuda_runtime.h>
@@ -55,11 +55,6 @@ __device__ __forceinline__ uint4 ld_ring16(const void* p) {
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
                : "l"(p));
   return r;
-}
-__device__ __forceinline__ void st_stream16(void* p, uint4 v) {
-  asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z),
-               "r"(v.w)
-               : "memory");
 }
 __device__ __forceinline__ uint64_t ld_acquire_u64(const void* p) {
   uint64_t v;
@@ -112,33 +107,48 @@ __device__ __forceinline__ void bulk_g2s(void* sdst, const void* gsrc, uint32_t 
 }
 // order this thread's earlier generic-proxy observations of global memory before its bulk copies
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+// shared -> global, byte-exact; completion is tracked in this thread's bulk groups.  gdst, ssrc 16-byte
+// aligned, bytes % 16 == 0.
+__device__ __forceinline__ void bulk_s2g(void* gdst, const void* ssrc, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(ssrc)),
+               "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 
-// Output vector i = source bytes [16 i + m, 16 i + m + 16) of the 16-byte aligned shared array
-// sv, m = 4 K + r/8.  Warp-cooperative, aligned 16-byte global stores.
+// In place: vector i of the 16-byte aligned shared array sv becomes source bytes [16 i + m, 16 i + m + 16),
+// m = 4 K + r/8 (a shift towards lower addresses).  Warp-cooperative, one 512-byte stripe at a time:
+// every lane reads its two vectors before any lane of the stripe writes; the next stripe's reads start
+// at the first vector this one did not write.
 template <int K>
-__device__ __forceinline__ void s2g_vectors(uint4* __restrict__ dv, const uint4* __restrict__ sv, uint32_t nvec,
-                                            uint32_t r, uint32_t lane) {
-#pragma unroll 4
-  for (uint32_t i = lane; i < nvec; i += 32) {
-    const uint4 A = sv[i], B = sv[i + 1];
-    uint32_t x0, x1, x2, x3, x4;
-    if (K == 0) { x0 = A.x; x1 = A.y; x2 = A.z; x3 = A.w; x4 = B.x; }
-    else if (K == 1) { x0 = A.y; x1 = A.z; x2 = A.w; x3 = B.x; x4 = B.y; }
-    else if (K == 2) { x0 = A.z; x1 = A.w; x2 = B.x; x3 = B.y; x4 = B.z; }
-    else { x0 = A.w; x1 = B.x; x2 = B.y; x3 = B.z; x4 = B.w; }
-    uint4 o;
-    o.x = __funnelshift_r(x0, x1, r);
-    o.y = __funnelshift_r(x1, x2, r);
-    o.z = __funnelshift_r(x2, x3, r);
-    o.w = __funnelshift_r(x3, x4, r);
-    st_stream16(dv + i, o);
+__device__ __forceinline__ void realign_vectors(uint4* sv, uint32_t nvec, uint32_t r, uint32_t lane) {
+  for (uint32_t j = 0; j < nvec; j += 32) {
+    const uint32_t i = j + lane;
+    uint4 o = make_uint4(0, 0, 0, 0);
+    if (i < nvec) {
+      const uint4 A = sv[i], B = sv[i + 1];
+      uint32_t x0, x1, x2, x3, x4;
+      if (K == 0) { x0 = A.x; x1 = A.y; x2 = A.z; x3 = A.w; x4 = B.x; }
+      else if (K == 1) { x0 = A.y; x1 = A.z; x2 = A.w; x3 = B.x; x4 = B.y; }
+      else if (K == 2) { x0 = A.z; x1 = A.w; x2 = B.x; x3 = B.y; x4 = B.z; }
+      else { x0 = A.w; x1 = B.x; x2 = B.y; x3 = B.z; x4 = B.w; }
+      o.x = __funnelshift_r(x0, x1, r);
+      o.y = __funnelshift_r(x1, x2, r);
+      o.z = __funnelshift_r(x2, x3, r);
+      o.w = __funnelshift_r(x3, x4, r);
+    }
+    __syncwarp();
+    if (i < nvec) sv[i] = o;
   }
 }
 
 // Warp-cooperative copy of n bytes from shared memory (16-byte aligned base `sbase`, byte offset
-// `soff`) to global memory at any alignment.  The stage holds at least one 16-byte block past the
-// last source byte's block start, so vector i+1 is always readable.
-__device__ __forceinline__ void smem_to_global(uint8_t* dst, const uint8_t* sbase, uint32_t soff, uint32_t n,
+// `soff`) to global memory at any alignment.  The <16-byte edges are stored byte by byte; the
+// aligned interior is realigned in place to the destination's phase and lane 0 issues one bulk store
+// for it (committed by the caller).  The stage holds at least one 16-byte block past the last source
+// byte's block start, so vector i+1 is always readable.  Bytes of the stage below soff + n may be
+// overwritten; the bytes from the block of soff + n on are left as they were.
+__device__ __forceinline__ void smem_to_global(uint8_t* dst, uint8_t* sbase, uint32_t soff, uint32_t n,
                                                uint32_t lane) {
   if (n == 0) return;
   uint32_t head = (16 - (uint32_t)(reinterpret_cast<uintptr_t>(dst) & 15)) & 15;
@@ -147,37 +157,40 @@ __device__ __forceinline__ void smem_to_global(uint8_t* dst, const uint8_t* sbas
   const uint32_t tail = n - head - (nvec << 4);
   if (lane < head) dst[lane] = sbase[soff + lane];
   if (lane < tail) dst[head + (nvec << 4) + lane] = sbase[soff + head + (nvec << 4) + lane];
+  if (nvec == 0) return;
   const uint32_t vs = soff + head, m = vs & 15;
-  const uint4* sv = reinterpret_cast<const uint4*>(sbase + (vs - m));
-  uint4* dv = reinterpret_cast<uint4*>(dst + head);
-  if (m == 0) {
-#pragma unroll 4
-    for (uint32_t i = lane; i < nvec; i += 32) st_stream16(dv + i, sv[i]);
-    return;
+  uint4* sv = reinterpret_cast<uint4*>(sbase + (vs - m));
+  if (m != 0) {
+    __syncwarp();  // the edge bytes are read before the realignment overwrites them
+    const uint32_t r = (m & 3) * 8;
+    switch (m >> 2) {
+      case 0: realign_vectors<0>(sv, nvec, r, lane); break;
+      case 1: realign_vectors<1>(sv, nvec, r, lane); break;
+      case 2: realign_vectors<2>(sv, nvec, r, lane); break;
+      default: realign_vectors<3>(sv, nvec, r, lane); break;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic writes -> the bulk store's reads
+    __syncwarp();
   }
-  const uint32_t r = (m & 3) * 8;
-  switch (m >> 2) {
-    case 0: s2g_vectors<0>(dv, sv, nvec, r, lane); break;
-    case 1: s2g_vectors<1>(dv, sv, nvec, r, lane); break;
-    case 2: s2g_vectors<2>(dv, sv, nvec, r, lane); break;
-    default: s2g_vectors<3>(dv, sv, nvec, r, lane); break;
-  }
+  if (lane == 0) bulk_s2g(dst + head, sv, nvec << 4);
 }
 
-// Warp-cooperative zero fill of n bytes at p (any alignment).
-__device__ __forceinline__ void coop_zero(uint8_t* p, uint64_t n, uint32_t lane) {
+// Warp-cooperative zero fill of n bytes at p (any alignment): byte stores at the <16-byte edges, bulk
+// stores from the zero block `zero` (kZeroBytes of shared memory) for the aligned interior, issued by
+// lane 0 (committed by the caller).
+constexpr uint32_t kZeroBytes = 1024;
+__device__ __forceinline__ void coop_zero(uint8_t* p, uint64_t n, const uint8_t* zero, uint32_t lane) {
   if (n == 0) return;
   uint64_t head = (16 - (reinterpret_cast<uintptr_t>(p) & 15)) & 15;
   if (head > n) head = n;
   if (lane < head) p[lane] = 0;
   p += head;
   n -= head;
-  const uint64_t nvec = n >> 4;
-  uint4* d = reinterpret_cast<uint4*>(p);
-  const uint4 z = make_uint4(0, 0, 0, 0);
-  for (uint64_t i = lane; i < nvec; i += 32) st_stream16(d + i, z);
-  const uint64_t done = nvec << 4;
-  if (lane < n - done) p[done + lane] = 0;
+  const uint64_t body = n & ~15ull;
+  if (lane < n - body) p[body + lane] = 0;
+  if (lane == 0)
+    for (uint64_t o = 0; o < body; o += kZeroBytes)
+      bulk_s2g(p + o, zero, body - o < kZeroBytes ? (uint32_t)(body - o) : kZeroBytes);
 }
 
 // GetReadableSize / HasMessage of a pair whose cursor is (head, remain)
@@ -289,6 +302,15 @@ struct PipeCtl {
   uint32_t op_done;
 };
 
+// Shared by every kernel of this file: the ticket ring, the stage barriers, the zero block the Recv movers
+// clear from, and the stages (dynamic shared memory).
+struct PipeSmem {
+  WorkItem q[kQI];
+  PipeCtl ctl;
+  uint64_t bars[kMovers * kDepth];
+  uint4 zero[kZeroBytes / 16];
+};
+
 __device__ __forceinline__ uint32_t ld_shared_volatile(const uint32_t* p) { return *(const volatile uint32_t*)p; }
 
 // producer side: wait for the slot of item `id`, fill it, publish
@@ -304,8 +326,10 @@ __device__ __forceinline__ void publish_item(WorkItem* q, uint32_t id, uint64_t 
   *(volatile uint32_t*)&slot->ready = id + 1;
 }
 
-__device__ __forceinline__ void movers_init(uint64_t* bars, uint32_t tid) {
-  if (tid < kMovers * kDepth) mbar_init(&bars[tid], 1);
+// Callers pass a __syncthreads before the movers run.
+__device__ __forceinline__ void movers_init(PipeSmem& pipe, uint32_t tid) {
+  if (tid < kMovers * kDepth) mbar_init(&pipe.bars[tid], 1);
+  for (uint32_t i = tid; i < kZeroBytes / 16; i += kThreads) pipe.zero[i] = make_uint4(0, 0, 0, 0);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -338,6 +362,8 @@ __device__ __forceinline__ void mover_run(const Move& mv, WorkItem* q, PipeCtl* 
         if (st == 1) {
           __threadfence_block();
           const uint32_t s = tail % kDepth;
+          // the stage is refilled only once the bulk stores of its previous item have read it
+          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
           mv.issue(slot->a, slot->n, stages + s * kStageBytes, &bars[s]);
           st |= si << 8;
           ticket = atomicAdd(&ctl->next, 1u);  // claim ahead
@@ -370,9 +396,19 @@ __device__ __forceinline__ void mover_run(const Move& mv, WorkItem* q, PipeCtl* 
     const uint32_t in = w->n;
     mv.process(ia, ib, ic, in, stages + s * kStageBytes, lane);
     __syncwarp();  // every lane is done with the stage and the descriptor before they are reused
-    if (lane == 0) *(volatile uint32_t*)&w->ready = 0;  // the ticket-ring slot may be refilled
+    if (lane == 0) {
+      bulk_commit();                            // the item's bulk stores: one group
+      *(volatile uint32_t*)&w->ready = 0;  // the ticket-ring slot may be refilled
+    }
     head++;
   }
+  // The segment's bulk stores are complete and ordered before the generic-proxy fence and barrier that
+  // end the segment (footers, credit, the op's answer), so nobody sees those before the bytes.
+  if (lane == 0) {
+    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    fence_proxy_async_global();
+  }
+  __syncwarp();
 }
 
 // =========================================================================
@@ -675,22 +711,16 @@ struct SendMove {
     mbar_expect_tx(bar, len);
     bulk_g2s(stage, reinterpret_cast<const void*>(a - pre), len, bar);
   }
-  __device__ __forceinline__ void process(uint64_t a, uint64_t b, uint64_t c, uint32_t n, const uint8_t* stage,
+  __device__ __forceinline__ void process(uint64_t a, uint64_t b, uint64_t c, uint32_t n, uint8_t* stage,
                                           uint32_t lane) const {
     const uint32_t pre = (uint32_t)(a & 15);
     if (c != 0 && lane == 0) *reinterpret_cast<uint64_t*>(ring + ((b + cap - 8) & mask)) = c;  // AppendHeader
     uint64_t seg1 = cap - b;
     if (seg1 > n) seg1 = n;
+    // the first part only rewrites stage bytes below its end, where the second part's source starts
     smem_to_global(ring + b, stage, pre, (uint32_t)seg1, lane);
     if (n > seg1) smem_to_global(ring, stage, pre + (uint32_t)seg1, n - (uint32_t)seg1, lane);  // wrap: WR1 at remote+0
   }
-};
-
-// Shared by every kernel of this file: the ticket ring, the stage barriers and the stages.
-struct PipeSmem {
-  WorkItem q[kQI];
-  PipeCtl ctl;
-  uint64_t bars[kMovers * kDepth];
 };
 
 // One Send op (PairPollable::Send, or the rdma_flush loop around it) by the whole CTA.
@@ -806,7 +836,7 @@ __global__ void __launch_bounds__(kThreads, 2)
 k_send(PairDev* __restrict__ pairs, const SendOpDev* __restrict__ ops, OpResult* __restrict__ results) {
   extern __shared__ __align__(128) uint8_t stage_mem[];
   __shared__ PipeSmem pipe;
-  movers_init(pipe.bars, threadIdx.x);
+  movers_init(pipe, threadIdx.x);
   uint32_t phase_bits = 0;
   const SendOpDev op = ops[blockIdx.x];
   send_body(pairs, op, &results[blockIdx.x], pipe, stage_mem, phase_bits);
@@ -1101,6 +1131,7 @@ struct RecvMove {
   uint8_t* ring;
   uint8_t* dst;
   uint64_t cap, mask;
+  const uint8_t* zero;  // kZeroBytes of zeros in shared memory
   __device__ __forceinline__ void issue(uint64_t a, uint32_t n, uint8_t* stage, uint64_t* bar) const {
     const uint32_t pre = (uint32_t)(a & 15);
     const uint64_t start = a - pre;
@@ -1120,7 +1151,7 @@ struct RecvMove {
       bulk_g2s(stage + len1, ring, len2, bar);
     }
   }
-  __device__ __forceinline__ void process(uint64_t a, uint64_t b, uint64_t c, uint32_t n, const uint8_t* stage,
+  __device__ __forceinline__ void process(uint64_t a, uint64_t b, uint64_t c, uint32_t n, uint8_t* stage,
                                           uint32_t lane) const {
     // ---- clear-on-read: exactly what the item retired (its bytes are already in shared memory)
     const uint32_t zhead = (uint32_t)(c & 0xffff), ztail = (uint32_t)(c >> 16);
@@ -1128,8 +1159,8 @@ struct RecvMove {
     const uint64_t zl = (uint64_t)zhead + n + ztail;
     uint64_t z1 = cap - zs;
     if (z1 > zl) z1 = zl;
-    coop_zero(ring + zs, z1, lane);
-    if (zl > z1) coop_zero(ring, zl - z1, lane);
+    coop_zero(ring + zs, z1, zero, lane);
+    if (zl > z1) coop_zero(ring, zl - z1, zero, lane);
     // ---- scatter
     smem_to_global(dst + b, stage, (uint32_t)(a & 15), n, lane);
   }
@@ -1180,7 +1211,7 @@ __device__ __forceinline__ void recv_body(PairDev* __restrict__ pairs, const Rec
     if (warp == 0) {
       recv_produce_segment(op, ring, cap, SS, q, &ctl, lane);
     } else {
-      const RecvMove mv{ring, op.dst, cap, mask};
+      const RecvMove mv{ring, op.dst, cap, mask, reinterpret_cast<const uint8_t*>(pipe.zero)};
       mover_run(mv, q, &ctl, stage_mem + (warp - 1) * (kDepth * kStageBytes), &bars[(warp - 1) * kDepth], phase_bits, lane);
     }
     const bool credit = ld_shared_volatile(&SS.credit_flag) != 0;  // stable: the producer finished this segment
@@ -1223,7 +1254,7 @@ __global__ void __launch_bounds__(kThreads, 2)
 k_recv(PairDev* __restrict__ pairs, const RecvOpDev* __restrict__ ops, OpResult* __restrict__ results) {
   extern __shared__ __align__(128) uint8_t stage_mem[];
   __shared__ PipeSmem pipe;
-  movers_init(pipe.bars, threadIdx.x);
+  movers_init(pipe, threadIdx.x);
   uint32_t phase_bits = 0;
   const RecvOpDev op = ops[blockIdx.x];
   recv_body(pairs, op, &results[blockIdx.x], pipe, stage_mem, phase_bits);
@@ -2107,7 +2138,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_svc_big(SvcParams sp) {
   __shared__ uint32_t s_stop;
   __shared__ __align__(16) BigBox s_box;
   const uint32_t tid = threadIdx.x;
-  movers_init(pipe.bars, tid);
+  movers_init(pipe, tid);
   uint32_t phase_bits = 0;
   const int nboxes = sp.nowners * (int)kOwnBoxes;
   uint32_t idle = 0;
@@ -2284,7 +2315,7 @@ k_probe_copy(uint8_t* __restrict__ dst, uint8_t* __restrict__ src, uint64_t byte
   if (item_bytes > kChunk) item_bytes = kChunk;
   const uint32_t nitems = (uint32_t)(bytes_per_cta / item_bytes);
   if (tid < kQI) q[tid].ready = 0;
-  movers_init(bars, tid);
+  movers_init(pipe, tid);
   uint32_t phase_bits = 0;
   if (tid == 0) {
     ctl.next = 0;
@@ -2307,7 +2338,7 @@ k_probe_copy(uint8_t* __restrict__ dst, uint8_t* __restrict__ src, uint64_t byte
       *(volatile uint32_t*)&ctl.seg_done = 1;
     }
   } else if (zero_after) {
-    const RecvMove mv{sbase, d, kBig, kBig - 1};
+    const RecvMove mv{sbase, d, kBig, kBig - 1, reinterpret_cast<const uint8_t*>(pipe.zero)};
     mover_run(mv, q, &ctl, stage_mem + (warp - 1) * (kDepth * kStageBytes), &bars[(warp - 1) * kDepth], phase_bits, lane);
   } else {
     const SendMove mv{d, kBig, kBig - 1};
