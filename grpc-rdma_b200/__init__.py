@@ -89,6 +89,7 @@ _SIGS = {
     "b200_pair_writable": (C.c_uint64, [C.c_void_p]),
     "b200_pair_status": (C.c_int, [C.c_void_p]),
     "b200_pair_error": (C.c_char_p, [C.c_void_p]),
+    "b200_pair_stamped": (C.c_int, [C.c_void_p]),
     "b200_pair_wakeup_read_fd": (C.c_int, [C.c_void_p]),
     "b200_pair_consume_wakeup": (None, [C.c_void_p]),
     "b200_pair_get_state": (C.c_int, [C.c_void_p, C.POINTER(PairState)]),
@@ -225,6 +226,10 @@ class Pair:
     def error(self):
         return self.L.b200_pair_error(self.h).decode()
 
+    def stamped(self):
+        """True when the connected pair runs stamped ring frames (both ends offered B200_RING_STAMPED)."""
+        return self.L.b200_pair_stamped(self.h) == 1
+
     def wakeup_fd(self):
         return self.L.b200_pair_wakeup_read_fd(self.h)
 
@@ -320,12 +325,13 @@ def chttp2_slice_lens(message_bytes, max_frame=HTTP2_MAX_FRAME):
     return lens
 
 
-def frame_hbm_bytes(lens):
+def frame_hbm_bytes(lens, stamped=False):
     """Algorithmic HBM bytes for one pass of the slice list (DESIGN.md):
-    gather reads p and writes E(p); deframe reads E, writes p, clears E."""
+    gather reads p and writes E(p); deframe reads E, writes p, clears E
+    (stamped ring frames: reads E, writes p, no clear)."""
     tx = rx = 0
     for p in lens:
         e = 16 + ((p + 7) // 8) * 8
         tx += p + e
-        rx += e + p + e
+        rx += e + p + (0 if stamped else e)
     return tx, rx

@@ -64,6 +64,7 @@ struct Config {
   int poller_sleep_ms = 1000;            // GRPC_RDMA_POLLER_SLEEP_TIMEOUT_MS, config.cc:83-89
   int max_sge = 30;                      // ibv_device_attr.max_sge on the authors' HCA
   int send_coalesce = 0;                 // B200_SEND_COALESCE: one frame per Send call (DESIGN.md §2)
+  int ring_stamped = 0;                  // B200_RING_STAMPED: offer stamped ring frames at Connect (DESIGN.md §2)
 };
 
 // Address blob: same 48-byte layout as grpc_core::ibverbs::Address::addr_
@@ -74,10 +75,11 @@ struct AddrBlob {
   uint32_t _pad0;
   uint8_t gid[16];
   uint32_t tag;
-  uint32_t _pad1;
+  uint32_t _pad1;  // capability bits of this library (kBlob*); 0 in every blob written before they existed
   uint64_t ring_buffer_size;
 };
 static_assert(sizeof(AddrBlob) == B200_ADDRESS_BYTES, "address blob must stay 48 bytes");
+constexpr uint32_t kBlobStamped = 0x1;  // this end offers stamped ring frames
 
 struct b200_pair {
   int slot = -1;
@@ -102,6 +104,8 @@ struct b200_pair {
   std::chrono::steady_clock::time_point last_probe{};
   int max_sge = 30;  // captured at Init (what the kernels use for this pair)
   bool coalesce = false;  // B200_SEND_COALESCE, captured at Init like max_sge
+  bool stamp_offer = false;  // B200_RING_STAMPED at Init and a ring of <= kStampedMaxCap: the blob's kBlobStamped
+  bool stamped = false;      // negotiated at Connect: both ends offered stamped frames
   // service: payload bytes Recv has returned since the service started (the device keeps the same count;
   // an eagerly pushed frame is valid only while both agree), and the asynchronous Retire of the last
   // eagerly received frame, if it has not been confirmed yet
@@ -147,8 +151,6 @@ static void drain_retire(b200_pair* p);
 
 namespace {
 
-constexpr int kMaxPairs = 8192;
-
 struct Runtime {
   std::mutex mu;       // setup + single-call submit
   bool inited = false;
@@ -162,7 +164,7 @@ struct Runtime {
   cudaEvent_t send_done[kLanes] = {}, recv_done[kLanes] = {};
   cudaEvent_t join_up[kLanes] = {}, join_down[kLanes] = {};
   cudaEvent_t fork_event = nullptr;
-  PairDev* d_pairs = nullptr;
+  PairDev* d_pairs = nullptr;       // kMaxPairs rows, then the kMaxPairs PairSeq of pair_seq()
   PairMirror* h_mirrors = nullptr;  // pinned, mapped
   std::vector<b200_pair*> all_pairs;
   std::queue<b200_pair*> pool;
@@ -411,6 +413,7 @@ static int init_locked(int device) {
   r.cfg.max_sge = (int)env_long("GRPC_RDMA_MAX_SGE", 30);
   if (r.cfg.max_sge < 1 || r.cfg.max_sge > kMaxSgeLimit) r.cfg.max_sge = 30;
   r.cfg.send_coalesce = env_long("B200_SEND_COALESCE", 0) == 1 ? 1 : 0;
+  r.cfg.ring_stamped = env_long("B200_RING_STAMPED", 0) == 1 ? 1 : 0;
 
   if (!CU_OK(cudaStreamCreateWithFlags(&r.stream, cudaStreamNonBlocking))) return -1;
   if (!CU_OK(cudaStreamCreateWithFlags(&r.poll_stream, cudaStreamNonBlocking))) return -1;
@@ -421,8 +424,9 @@ static int init_locked(int device) {
       if (!CU_OK(cudaEventCreateWithFlags(e, cudaEventDisableTiming))) return -1;
   }
   if (!CU_OK(cudaEventCreateWithFlags(&r.fork_event, cudaEventDisableTiming))) return -1;
-  if (!CU_OK(cudaMalloc(&r.d_pairs, sizeof(PairDev) * kMaxPairs))) return -1;
-  if (!CU_OK(cudaMemset(r.d_pairs, 0, sizeof(PairDev) * kMaxPairs))) return -1;
+  const size_t table_bytes = (sizeof(PairDev) + sizeof(PairSeq)) * kMaxPairs;
+  if (!CU_OK(cudaMalloc(&r.d_pairs, table_bytes))) return -1;
+  if (!CU_OK(cudaMemset(r.d_pairs, 0, table_bytes))) return -1;
   if (!CU_OK(cudaHostAlloc(&r.h_mirrors, sizeof(PairMirror) * kMaxPairs, cudaHostAllocMapped | cudaHostAllocPortable)))
     return -1;
   memset(r.h_mirrors, 0, sizeof(PairMirror) * kMaxPairs);
@@ -541,6 +545,9 @@ extern "C" int b200_config_set(const char* key, const char* value) {
   } else if (k == "B200_SEND_COALESCE") {
     if (v != 0 && v != 1) return -1;
     r.cfg.send_coalesce = (int)v;
+  } else if (k == "B200_RING_STAMPED") {
+    if (v != 0 && v != 1) return -1;
+    r.cfg.ring_stamped = (int)v;
   } else {
     set_err("b200_config_set: unknown key " + k);
     return -1;
@@ -559,6 +566,7 @@ extern "C" int64_t b200_config_get(const char* key) {
   if (k == "GRPC_RDMA_POLLER_SLEEP_TIMEOUT_MS") return r.cfg.poller_sleep_ms;
   if (k == "GRPC_RDMA_MAX_SGE") return r.cfg.max_sge;
   if (k == "B200_SEND_COALESCE") return r.cfg.send_coalesce;
+  if (k == "B200_RING_STAMPED") return r.cfg.ring_stamped;
   return -1;
 }
 
@@ -655,8 +663,10 @@ extern "C" b200_pair* b200_pool_get(const char* id) {
   return it == r.id_pair.end() ? nullptr : it->second;
 }
 
-// the pair's max_sge word of PairDev: the mode rides in its top bit so the line stays 128 bytes
-static uint32_t sge_word(const b200_pair* p) { return (uint32_t)p->max_sge | (p->coalesce ? kSgeCoalesce : 0u); }
+// the pair's max_sge word of PairDev: the modes ride in its top bits so the line stays 128 bytes
+static uint32_t sge_word(const b200_pair* p) {
+  return (uint32_t)p->max_sge | (p->coalesce ? kSgeCoalesce : 0u) | (p->stamped ? kSgeStamped : 0u);
+}
 
 extern "C" void b200_pair_init(b200_pair* p) {
   if (!p || !ensure_init()) return;
@@ -692,6 +702,8 @@ extern "C" void b200_pair_init(b200_pair* p) {
   hd.status = B200_INITIALIZED;
   p->max_sge = r.cfg.max_sge;
   p->coalesce = r.cfg.send_coalesce != 0;
+  p->stamp_offer = r.cfg.ring_stamped != 0 && cap <= kStampedMaxCap;
+  p->stamped = false;
   hd.max_sge = sge_word(p);
   hd.peer_slot = -1;
   p->svc_delivered = 0;
@@ -701,6 +713,7 @@ extern "C" void b200_pair_init(b200_pair* p) {
   memset(p->mirror, 0, sizeof(PairMirror));
   bool ok = CU_OK(cudaMemsetAsync(p->ring, 0, cap, r.stream)) &&  // RingBufferPollable::Init
             CU_OK(cudaMemcpyAsync(&r.d_pairs[p->slot], &hd, sizeof(hd), cudaMemcpyHostToDevice, r.stream)) &&
+            CU_OK(cudaMemsetAsync(pair_seq(r.d_pairs, p->slot), 0, sizeof(PairSeq), r.stream)) &&
             CU_OK(cudaStreamSynchronize(r.stream));
   if (!ok) {
     p->error = t_err;
@@ -728,6 +741,7 @@ extern "C" void b200_pair_init(b200_pair* p) {
   memcpy(p->self.gid + 4, &r.dev, 4);          // which GPU
   memcpy(p->self.gid + 8, &p->slot, 4);        // which row of the connection table
   p->self.tag = B200_PAIR_TAG_POLLABLE;
+  p->self._pad1 = p->stamp_offer ? kBlobStamped : 0u;
   p->self.ring_buffer_size = cap;  // "used to check peer has the same size", pair.cc:107
   r.by_qpn[p->self.qpn] = p;
   p->peer_local = nullptr;
@@ -785,6 +799,9 @@ extern "C" int b200_pair_connect(b200_pair* p, const void* peer48, size_t n) {
     set_err(p->error);
     return 0;
   }
+  // stamped frames when both ends offer them: both compute the same AND, and a peer without the bit (any
+  // blob written before the bit existed) gets the reference format.  Set right before the setup line is written.
+  const bool stamped = p->stamp_offer && (p->peer._pad1 & kBlobStamped) != 0;
   uint32_t cookie;
   memcpy(&cookie, p->peer.gid, 4);
   if (cookie != r.cookie) {
@@ -829,6 +846,7 @@ extern "C" int b200_pair_connect(b200_pair* p, const void* peer48, size_t n) {
     hd.mirror = p->mirror;
     hd.peer_mirror = nullptr;
     hd.status = B200_CONNECTED;
+    p->stamped = stamped;
     hd.max_sge = sge_word(p);
     hd.peer_slot = -1;
     hd.wire = 1;  // system-scope fences: the ring is in another GPU's HBM, reached over NVLink
@@ -868,6 +886,7 @@ extern "C" int b200_pair_connect(b200_pair* p, const void* peer48, size_t n) {
   hd.mirror = p->mirror;
   hd.peer_mirror = q->mirror;
   hd.status = B200_CONNECTED;
+  p->stamped = stamped;
   hd.max_sge = sge_word(p);
   hd.peer_slot = q->slot;
   hd.wire = 0;
@@ -962,6 +981,9 @@ extern "C" enum b200_status b200_pair_status(b200_pair* p) {
   return (enum b200_status)p->status;
 }
 extern "C" const char* b200_pair_error(const b200_pair* p) { return p ? p->error.c_str() : ""; }
+extern "C" int b200_pair_stamped(const b200_pair* p) {
+  return p && p->stamped && (p->status == B200_CONNECTED || p->status == B200_HALF_CLOSED) ? 1 : 0;
+}
 extern "C" int b200_pair_wakeup_read_fd(b200_pair* p) { return p ? p->wakeup_fd : -1; }
 extern "C" void b200_pair_consume_wakeup(b200_pair* p) {
   if (!p) return;

@@ -91,6 +91,12 @@ const char* b200_last_error(void);
  * credit runs out (max_sge does not apply; zero-length slices are skipped, not a stop).
  * The peer's receive side is unchanged and needs no negotiation (DESIGN.md §2).
  * Like GRPC_RDMA_MAX_SGE it is captured into the pair at b200_pair_init.
+ * B200_RING_STAMPED (0 / 1, default 0): 1 = the pair offers stamped ring frames
+ * (header = p | t << 40 with a per-frame stamp t, footer = ~header; the receiver
+ * never clears what it retires).  Captured at b200_pair_init and offered in the
+ * address blob when the ring is <= 256 MiB; a connection runs stamped frames only
+ * when both ends offered them, otherwise the reference format (DESIGN.md §2).
+ * Return values, cursors and the delivered stream are those of the reference.
  * The environment is read at b200_init; b200_config_set overrides afterwards
  * (affects pairs initialised later).  Returns 0 / -1 (unknown key, bad value). */
 int b200_config_set(const char* key, const char* value);
@@ -145,6 +151,9 @@ uint64_t b200_pair_writable(const b200_pair* p);
 /* get_status, pair.cc:349-375; get_error, pair.cc:643 */
 enum b200_status b200_pair_status(b200_pair* p);
 const char* b200_pair_error(const b200_pair* p);
+/* 1 when the connected pair runs stamped ring frames (both ends offered
+ * B200_RING_STAMPED), 0 otherwise. */
+int b200_pair_stamped(const b200_pair* p);
 /* get_wakeup_fd()->read_fd, pair.cc:377: an eventfd the engine registers in
  * epoll with tag ptr|2 (ev_epollex_rdma_bpev_linux.cc:725-741). */
 int b200_pair_wakeup_read_fd(b200_pair* p);
