@@ -279,7 +279,12 @@ int b200_pairs_recv(const b200_recv_op* ops, size_t nops, int flags, uint64_t* d
 /* One event-loop pass: all ready Sends and Recvs posted together, waited for together (what
  * pollable_process_events does closure by closure, ev_epollex_rdma_bpev_linux.cc:977-1066).  With the service
  * running nothing is launched: every op is a command of its pair's owner queue, slices (any host memory;
- * unregistered slices are staged) and destinations (GPU-addressable) are used in place.  0 on success. */
+ * unregistered slices are staged) and destinations (GPU-addressable) are used in place.  0 on success.
+ * At most one Send op and one Recv op of a pair may be in flight at a time -- within one pass and across threads
+ * (the ContentAssertion rule above): a pair's Send and Recv run side by side on the pool, but two Sends (or two
+ * Recvs) of one pair would overlap too, because an owner hands a job to the pool after reaping only the jobs that
+ * have already finished.  A pass that holds the Send of one direction of a connection and the Recv of the same
+ * direction runs both concurrently: their per-op counts depend on timing, the delivered stream does not. */
 int b200_pairs_submit(const b200_send_op* sops, size_t ns, uint64_t* accepted, const b200_recv_op* rops, size_t nr,
                       uint64_t* delivered, int flags);
 
