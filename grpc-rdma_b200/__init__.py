@@ -23,6 +23,7 @@ ENDPOINT_LIB_PATH = os.path.join(PKG_DIR, "lib", "libb200_endpoint.so")
 ENDPOINT_HEADER = os.path.join(ROOT, "include", "b200_endpoint.h")
 
 ADDRESS_BYTES = 48
+DEV_PAIR_BYTES = 64  # sizeof(b200_dev_pair)
 ONE_CALL, UNTIL_BLOCKED, ASYNC, ZEROCOPY = 0, 1, 2, 4
 EV_READABLE, EV_WRITABLE = 0x1, 0x4
 STATUS = ["UNINITIALIZED", "INITIALIZED", "CONNECTED", "HALF_CLOSED", "DISCONNECTED", "ERROR"]
@@ -121,6 +122,9 @@ _SIGS = {
     "b200_probe_copy": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_uint32,
                                   C.c_uint32, C.c_uint32, C.c_void_p]),
     "b200_launch_count": (C.c_uint64, []),
+    "b200_pair_device_claim": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "b200_pair_device_release": (C.c_int, [C.c_void_p]),
+    "b200_pair_device_owned": (C.c_int, [C.c_void_p]),
 }
 
 _lib = None
@@ -249,6 +253,22 @@ class Pair:
         if self.L.b200_pair_copy_ring(self.h, out.ctypes.data, out.size) != 0:
             raise RuntimeError(last_error())
         return out
+
+    def device_claim(self):
+        """Hand this end to the caller's kernels (include/b200_device.cuh): returns the 64-byte b200_dev_pair
+        handle.  Host calls on this end are refused until device_release()."""
+        buf = C.create_string_buffer(DEV_PAIR_BYTES)
+        if self.L.b200_pair_device_claim(self.h, buf) != 0:
+            raise RuntimeError("b200_pair_device_claim failed: " + last_error())
+        return buf.raw
+
+    def device_release(self):
+        """Give the end back to the host; the kernels that used the handle must have finished."""
+        if self.L.b200_pair_device_release(self.h) != 0:
+            raise RuntimeError("b200_pair_device_release failed: " + last_error())
+
+    def device_owned(self):
+        return self.L.b200_pair_device_owned(self.h) == 1
 
     def disconnect(self):
         self.L.b200_pair_disconnect(self.h)

@@ -115,7 +115,36 @@ struct b200_pair {
   uint64_t retire_ticket = 0;
   std::atomic<uint32_t> retire_owed{0};  // size of an eagerly received frame whose Retire has not been posted yet:
                                          // it rides on the pair's next Send, or is posted by whoever looks next
+  // device API (b200_pair_device_claim): host ops on this end are refused while it is set.  A host op counts
+  // itself in host_ops before it looks at device_owned, the claim sets device_owned before it looks at host_ops,
+  // so one of the two always sees the other.
+  std::atomic<bool> device_owned{false};
+  std::atomic<int> host_ops{0};
 };
+
+static const char* const kDeviceOwnedRefusal =
+    "the pair is device-owned (b200_pair_device_claim): host operations are refused until the release";
+// a host op on pair p for as long as it lives (refused: !ok, p->error says why)
+struct HostOp {
+  b200_pair* p;
+  bool ok;
+  explicit HostOp(b200_pair* pp) : p(pp) {
+    p->host_ops.fetch_add(1);
+    ok = !p->device_owned.load();
+    if (!ok) p->error = kDeviceOwnedRefusal;
+  }
+  ~HostOp() { p->host_ops.fetch_sub(1); }
+};
+static bool any_device_owned(const b200_pair* const* pairs, size_t n, size_t stride_bytes, const char* who) {
+  for (size_t i = 0; i < n; i++) {
+    const b200_pair* p = *(const b200_pair* const*)((const char*)pairs + i * stride_bytes);
+    if (p && p->device_owned.load()) {
+      t_err = std::string(who) + ": a pair of the batch is device-owned (b200_pair_device_claim)";
+      return true;
+    }
+  }
+  return false;
+}
 
 constexpr int kLanes = 16;  // max internal lanes of the host-staged path (B200_LANES, default 8)
 
@@ -144,6 +173,11 @@ struct b200_batch {
   uint8_t* d_stage = nullptr;
   std::vector<int> perm;  // perm[k] = caller's index of device op k
   std::vector<b200_pair*> pairs;  // the pairs of a Recv batch (service: their eager records go stale at launch)
+  std::vector<b200_pair*> op_pairs;  // the pair of every op: refused at launch when device-owned, and counted as
+                                     // host ops of them from the launch until the results are collected
+  bool counted = false;
+  std::vector<SendOpDev> h_sops;  // host copies of the descriptors: B200_BATCH_CONCURRENT is added at launch when
+  std::vector<RecvOpDev> h_rops;  // a peer has been claimed since the batch was prepared
   LanePlan lanes[kLanes];
 };
 
@@ -224,6 +258,10 @@ struct Runtime {
   // bumped whenever the host changes pair lines on the device or launches kernels beside the service; every
   // command carries it (SvcCmd.op >> 8) and an owner warp that sees a new value drops its cached lines
   std::atomic<uint32_t> svc_gen{1};
+  // slots claimed by b200_pair_device_claim: a command for a connection with a claimed end carries
+  // B200_BATCH_CONCURRENT, so the owner warp reads that connection's lines fresh and publishes its mirrors under the
+  // per-pair locks (a user kernel changes them meanwhile)
+  std::atomic<uint8_t> dev_slot[kMaxPairs] = {};
   uint32_t svc_ready_head = 0;      // next stream index the host expects (under scan_mu)
   std::vector<uint16_t> svc_level;  // events pending per slot, as last reported by the device poller
   std::mutex grave_mu;
@@ -622,6 +660,8 @@ extern "C" int b200_stream_sync(void* stream) {
 
 // ================================================================ pool / pair
 
+static void device_release_locked(Runtime& r, b200_pair* p);
+
 extern "C" b200_pair* b200_pool_take(const char* id) {
   if (!ensure_init()) return nullptr;
   Runtime& r = R();
@@ -651,6 +691,7 @@ extern "C" void b200_pool_putback(b200_pair* p) {
   if (!p) return;
   Runtime& r = R();
   std::lock_guard<std::mutex> lk(r.mu);
+  device_release_locked(r, p);
   auto it = r.id_pair.find(p->id);
   if (it != r.id_pair.end() && it->second == p) r.id_pair.erase(it);
   r.pool.push(p);
@@ -672,6 +713,7 @@ extern "C" void b200_pair_init(b200_pair* p) {
   if (!p || !ensure_init()) return;
   Runtime& r = R();
   std::lock_guard<std::mutex> lk(r.mu);
+  device_release_locked(r, p);
   // pair.cc:88-89: only from Uninitialized / Error / Disconnected
   if (!(p->status == B200_UNINITIALIZED || p->status == B200_ERROR || p->status == B200_DISCONNECTED)) return;
   cudaSetDevice(r.dev);
@@ -905,6 +947,7 @@ extern "C" void b200_pair_disconnect(b200_pair* p) {
   if (!p || !R().inited) return;
   Runtime& r = R();
   std::lock_guard<std::mutex> lk(r.mu);
+  device_release_locked(r, p);
   if (p->status == B200_UNINITIALIZED || p->status == B200_DISCONNECTED) return;  // pair.cc:326-327
   drain_retire(p);
   cudaSetDevice(r.dev);
@@ -1152,6 +1195,9 @@ static bool svc_try_post(Runtime& r, int q, Fill fill, uint64_t* ticket) {
   SvcCmd* c = &r.svc_cmds[e];
   c->nreal = 0;
   fill(c, r.svc_slices + e * (kSvcSliceArea + 1));
+  const int s0 = c->slot & 0xffff, s1 = (c->slot >> 16) - 1;
+  if ((s0 < kMaxPairs && r.dev_slot[s0].load()) || (s1 >= 0 && s1 < kMaxPairs && r.dev_slot[s1].load()))
+    c->flags |= B200_BATCH_CONCURRENT;
   c->op = (c->op & 0xffu) | ((r.svc_gen.load(std::memory_order_acquire) & 0xffffffu) << 8);
   std::atomic_thread_fence(std::memory_order_release);
   *(volatile uint32_t*)&c->stamp2 = (uint32_t)(t + 1);
@@ -1474,6 +1520,123 @@ static uint64_t svc_recv(Runtime& r, b200_pair* p, void* dst, uint64_t cap) {
   return bytes;
 }
 
+// ================================================================ device API
+
+// The host-visible mirror of p from the device state (readiness as rx_probe computes it)
+static void republish_mirror(Runtime& r, b200_pair* p) {
+  PairDev hd;
+  PairSeq sq;
+  if (!CU_OK(cudaMemcpy(&hd, &r.d_pairs[p->slot], sizeof(hd), cudaMemcpyDeviceToHost)) ||
+      !CU_OK(cudaMemcpy(&sq, pair_seq(r.d_pairs, p->slot), sizeof(sq), cudaMemcpyDeviceToHost)))
+    return;
+  uint32_t hm = 0;
+  uint64_t rd = 0;
+  if (hd.remain > 0) {
+    hm = 1;
+    rd = hd.remain;
+  } else if (hd.ring) {
+    const uint32_t st = (hd.max_sge & kSgeStamped) ? stamp_of(sq.rx) : 0;
+    uint64_t hdr = 0, foot = 0;
+    if (!CU_OK(cudaMemcpy(&hdr, hd.ring + hd.head, 8, cudaMemcpyDeviceToHost))) return;
+    hm = hdr != 0;
+    const uint64_t len = frame_present(hdr, hd.cap, st);
+    if (len && CU_OK(cudaMemcpy(&foot, hd.ring + ((hd.head + 8 + round_up8(len)) & (hd.cap - 1)), 8,
+                                cudaMemcpyDeviceToHost)) && foot == frame_footer(hdr, st))
+      rd = len;
+    if (st) hm = rd != 0;
+  }
+  volatile PairMirror* m = p->mirror;
+  m->head = hd.head;
+  m->moving_head = hd.moving_head;
+  m->remain = hd.remain;
+  m->acc = hd.acc;
+  m->readable = rd;
+  m->has_message = hm;
+  m->remote_tail = hd.remote_tail;
+  m->credit_head = hd.credit_head;
+  m->partial_write = hd.partial_write;
+  m->peer_exit = hd.credit_exit;
+}
+
+extern "C" int b200_pair_device_claim(b200_pair* p, b200_dev_pair* out) {
+  if (!p || !out || !ensure_init()) {
+    set_err("b200_pair_device_claim: no pair / no output / no CUDA device");
+    return -1;
+  }
+  Runtime& r = R();
+  if (p->status != B200_CONNECTED) {
+    set_err("b200_pair_device_claim: the pair is not connected");
+    return -1;
+  }
+  drain_retire(p);
+  bool was = false;
+  if (!p->device_owned.compare_exchange_strong(was, true)) {
+    set_err("b200_pair_device_claim: the pair is already device-owned");
+    return -1;
+  }
+  if (p->host_ops.load() != 0) {
+    p->device_owned = false;
+    set_err("b200_pair_device_claim: host operations on the pair are in flight");
+    return -1;
+  }
+  drain_retire(p);  // (an eager Recv that finished between the first drain and the claim)
+  {
+    std::lock_guard<std::mutex> lk(r.mu);
+    r.dev_slot[p->slot] = 1;
+    if (r.svc_running.load()) memset((void*)&r.svc_erec[p->slot], 0, sizeof(EagerRec));  // no eager Recv any more
+    r.svc_gen++;
+    memset(out, 0, sizeof(*out));
+    out->table = r.d_pairs;
+    out->seq = pair_seq(r.d_pairs, 0);
+    out->mirrors = r.h_mirrors;
+    out->slot = p->slot;
+    out->wire = p->remote ? 1 : 0;
+  }
+  if (r.svc_running.load()) {
+    // the connection's queue is in order: once this no-op is answered, every command of the peer posted before the
+    // claim has run, and the owner has seen the new generation (its cached lines of the connection are gone)
+    const int q = owner_of(r, p);
+    const uint64_t t = svc_post(r, q, [&](SvcCmd* c, SliceDev*) {
+      c->op = kSvcNop;
+      c->slot = slot_word(p);
+      c->flags = B200_BATCH_ONE_CALL;
+    });
+    svc_wait(r, q, t, nullptr, nullptr);
+  }
+  return 0;
+}
+
+// caller holds r.mu.  The device Recv calls do not count in the service's delivered counts (host and device
+// agree on them still); the eager record may have been pushed from a stale view: it is dropped.
+static void device_release_locked(Runtime& r, b200_pair* p) {
+  if (!p->device_owned.load()) return;
+  cudaSetDevice(r.dev);
+  if (r.svc_running.load()) {
+    const PairSvc fresh{p->svc_delivered, ~0ull};
+    memset((void*)&r.svc_erec[p->slot], 0, sizeof(EagerRec));
+    cudaMemcpyAsync(&r.d_svc_psvc[p->slot], &fresh, sizeof(fresh), cudaMemcpyHostToDevice, r.stream);
+    cudaStreamSynchronize(r.stream);
+  }
+  republish_mirror(r, p);
+  r.svc_gen++;
+  r.dev_slot[p->slot] = 0;
+  p->device_owned = false;
+  if (p->error == kDeviceOwnedRefusal) p->error.clear();
+}
+
+extern "C" int b200_pair_device_release(b200_pair* p) {
+  if (!p || !p->device_owned.load()) {
+    set_err("b200_pair_device_release: the pair is not device-owned");
+    return -1;
+  }
+  Runtime& r = R();
+  std::lock_guard<std::mutex> lk(r.mu);
+  device_release_locked(r, p);
+  return 0;
+}
+
+extern "C" int b200_pair_device_owned(const b200_pair* p) { return p && p->device_owned.load() ? 1 : 0; }
+
 // ================================================================ single call
 
 static bool ensure_bounce(uint8_t** buf, uint64_t* cap, uint64_t need) {
@@ -1491,7 +1654,11 @@ static bool ensure_bounce(uint8_t** buf, uint64_t* cap, uint64_t need) {
 // call; here it would be a launch per spin.  When the host-visible mirror already shows that the
 // call cannot accept a byte (no credit for even one frame and the partial-write flag already set),
 // the answer and the resulting state are exactly those of the kernel, so no kernel runs.
+// The mirror short-cuts below are not taken when a user kernel drives the other end (b200_pair_device_claim): its
+// warps and ours publish the mirror concurrently, so the answer comes from the device state instead.
+static bool peer_device_owned(const b200_pair* p) { return p->peer_local && p->peer_local->device_owned.load(); }
 static bool send_is_a_no_op(const b200_pair* p) {
+  if (peer_device_owned(p)) return false;
   volatile PairMirror* m = p->mirror;
   if (!m->partial_write) return false;
   const uint64_t fr = free_size(p->cap, m->credit_head, m->remote_tail);
@@ -1502,6 +1669,8 @@ static bool send_is_a_no_op(const b200_pair* p) {
 extern "C" uint64_t b200_pair_send(b200_pair* p, const b200_slice* slices, size_t n, size_t byte_idx) {
   if (!p || !ensure_init()) return 0;
   Runtime& r = R();
+  const HostOp op(p);
+  if (!op.ok) return 0;
   if (p->peer_dead.load()) return 0;  // nobody owns the remote ring any more: get_status reports HalfClosed
   if (p->status == B200_CONNECTED && n) {
     if (p->peer_local) drain_retire(p->peer_local);  // its Retire may be about to return credit
@@ -1558,7 +1727,9 @@ extern "C" uint64_t b200_pair_send(b200_pair* p, const b200_slice* slices, size_
     nsl++;
   }
   r.h_sop->slot = p->slot;
-  r.h_sop->flags = B200_BATCH_ONE_CALL;
+  // a device-owned peer publishes its mirror fields under the per-pair lock: so must we
+  const bool conc = p->peer_local && p->peer_local->device_owned.load();
+  r.h_sop->flags = B200_BATCH_ONE_CALL | (conc ? B200_BATCH_CONCURRENT : 0);
   r.h_sop->slices = r.h_slices;
   r.h_sop->nslices = nsl;
   r.h_sop->nreal = look;
@@ -1578,9 +1749,13 @@ extern "C" uint64_t b200_pair_send(b200_pair* p, const b200_slice* slices, size_
 extern "C" uint64_t b200_pair_recv(b200_pair* p, void* dst, uint64_t cap) {
   if (!p || !ensure_init()) return 0;
   Runtime& r = R();
+  const HostOp op(p);
+  if (!op.ok) return 0;
   drain_retire(p);
   // same reasoning for a Recv on a ring the mirror shows empty: it delivers nothing, changes nothing
-  if (p->status == B200_CONNECTED && !p->remote && ((volatile PairMirror*)p->mirror)->has_message == 0) return 0;
+  if (p->status == B200_CONNECTED && !p->remote && !peer_device_owned(p) &&
+      ((volatile PairMirror*)p->mirror)->has_message == 0)
+    return 0;
   if (r.svc_running.load()) {
     if (p->status != B200_CONNECTED || cap == 0) return 0;
     return svc_recv(r, p, dst, cap);
@@ -1597,7 +1772,8 @@ extern "C" uint64_t b200_pair_recv(b200_pair* p, void* dst, uint64_t cap) {
     kdst = r.bounce_rx;
   }
   r.h_rop->slot = p->slot;
-  r.h_rop->flags = B200_BATCH_ONE_CALL;
+  const bool conc = p->peer_local && p->peer_local->device_owned.load();
+  r.h_rop->flags = B200_BATCH_ONE_CALL | (conc ? B200_BATCH_CONCURRENT : 0);
   r.h_rop->dst = kdst;
   r.h_rop->cap = kcap;
   r.h_res->bytes = 0;
@@ -1675,6 +1851,9 @@ static void push_h2d(std::vector<CopyRun>& out, uint8_t* stage, const uint8_t* s
 
 static b200_batch* prepare_common(int kind, const void* ops_v, size_t nops, int flags) {
   if (!ensure_init()) return nullptr;
+  if (any_device_owned((const b200_pair* const*)ops_v, nops, kind == 0 ? sizeof(b200_send_op) : sizeof(b200_recv_op),
+                       "b200_batch_prepare"))
+    return nullptr;
   Runtime& r = R();
   cudaSetDevice(r.dev);
   b200_batch* b = new b200_batch();
@@ -1727,6 +1906,7 @@ static b200_batch* prepare_common(int kind, const void* ops_v, size_t nops, int 
     for (size_t i = 0; i < nops; i++) b->perm[i] = (int)i;
   }
   const uint32_t kflags = (uint32_t)(flags & (B200_BATCH_UNTIL_BLOCKED | B200_BATCH_CONCURRENT));
+  for (size_t k = 0; ok && k < nops; k++) b->op_pairs.push_back(kind == 0 ? sops[b->perm[k]].pair : rops[b->perm[k]].pair);
   if (ok && kind == 0) {
     size_t total_slices = 0;
     for (size_t i = 0; i < nops; i++) total_slices += sops[i].nslices;
@@ -1776,6 +1956,7 @@ static b200_batch* prepare_common(int kind, const void* ops_v, size_t nops, int 
     }
     ok = ok && CU_OK(cudaMemcpy(b->d_slices, hs.data(), sizeof(SliceDev) * hs.size(), cudaMemcpyHostToDevice)) &&
          CU_OK(cudaMemcpy(b->d_ops, h.data(), sizeof(SendOpDev) * (nops ? nops : 1), cudaMemcpyHostToDevice));
+    b->h_sops.swap(h);
   } else if (ok) {
     std::vector<RecvOpDev> h(nops ? nops : 1);
     ok = CU_OK(cudaMalloc(&b->d_ops, sizeof(RecvOpDev) * (nops ? nops : 1)));
@@ -1803,6 +1984,7 @@ static b200_batch* prepare_common(int kind, const void* ops_v, size_t nops, int 
       }
     }
     ok = ok && CU_OK(cudaMemcpy(b->d_ops, h.data(), sizeof(RecvOpDev) * (nops ? nops : 1), cudaMemcpyHostToDevice));
+    b->h_rops.swap(h);
   }
   ok = ok && CU_OK(cudaMalloc(&b->d_results, sizeof(OpResult) * (nops ? nops : 1))) &&
        CU_OK(cudaHostAlloc(&b->h_results, sizeof(OpResult) * (nops ? nops : 1), cudaHostAllocPortable));
@@ -1848,10 +2030,41 @@ extern "C" int b200_lanes_join(void* stream) {
   return 0;
 }
 
+// a device-owned peer publishes its mirror fields under the per-pair locks: so must the batch's kernels
+static bool batch_make_concurrent(b200_batch* b) {
+  bool need = false;
+  for (const b200_pair* p : b->op_pairs) need = need || (p->peer_local && p->peer_local->device_owned.load());
+  if (!need || (b->flags & B200_BATCH_CONCURRENT)) return true;
+  b->flags |= B200_BATCH_CONCURRENT;
+  if (b->kind == 0) {
+    for (SendOpDev& o : b->h_sops) o.flags |= kFlagConcurrent;
+    return CU_OK(cudaMemcpy(b->d_ops, b->h_sops.data(), sizeof(SendOpDev) * b->h_sops.size(), cudaMemcpyHostToDevice));
+  }
+  for (RecvOpDev& o : b->h_rops) o.flags |= kFlagConcurrent;
+  return CU_OK(cudaMemcpy(b->d_ops, b->h_rops.data(), sizeof(RecvOpDev) * b->h_rops.size(), cudaMemcpyHostToDevice));
+}
+static void batch_uncount(b200_batch* b) {
+  if (!b->counted) return;
+  for (b200_pair* p : b->op_pairs) p->host_ops.fetch_sub(1);
+  b->counted = false;
+}
+
 extern "C" int b200_batch_launch(b200_batch* b, void* stream) {
   if (!b) return -1;
   Runtime& r = R();
   if (b->nops == 0) return 0;
+  // from here until its results are collected the batch is a host op of each of its pairs (counted first, then the
+  // ownership looked at: see HostOp)
+  if (!b->counted) {
+    for (b200_pair* p : b->op_pairs) p->host_ops.fetch_add(1);
+    b->counted = true;
+  }
+  if (any_device_owned((const b200_pair* const*)b->op_pairs.data(), b->op_pairs.size(), sizeof(b200_pair*),
+                       "b200_batch_launch")) {
+    batch_uncount(b);
+    return -1;
+  }
+  if (!batch_make_concurrent(b)) return -1;
   if (r.svc_running.load()) r.svc_gen++;  // kernels beside the service change pair lines behind the owners' caches
   if (b->kind == 1 && r.svc_running.load()) {
     // frames are about to be consumed behind the service's back: whatever it pushed eagerly for these pairs
@@ -1916,6 +2129,7 @@ extern "C" int b200_batch_results(b200_batch* b, uint64_t* out, void* stream) {
     return -1;
   if (out)
     for (int k = 0; k < b->nops; k++) out[b->perm[k]] = b->h_results[k].bytes;
+  batch_uncount(b);
   return 0;
 }
 
@@ -1927,6 +2141,7 @@ extern "C" int b200_batch_calls(b200_batch* b, uint64_t* out) {
 
 extern "C" void b200_batch_destroy(b200_batch* b) {
   if (!b) return;
+  batch_uncount(b);
   rt_free(b->d_ops, 0);
   rt_free(b->d_slices, 0);
   rt_free(b->d_results, 0);
@@ -1961,6 +2176,22 @@ extern "C" int b200_pairs_submit(const b200_send_op* sops, size_t ns, uint64_t* 
                                  size_t nr, uint64_t* delivered, int flags) {
   if (!ensure_init()) return -1;
   Runtime& r = R();
+  // the pass counts as a host op of each of its pairs until it returns
+  static thread_local std::vector<b200_pair*> held;
+  held.clear();
+  for (size_t i = 0; i < ns; i++)
+    if (sops[i].pair) held.push_back(sops[i].pair);
+  for (size_t i = 0; i < nr; i++)
+    if (rops[i].pair) held.push_back(rops[i].pair);
+  for (b200_pair* p : held) p->host_ops.fetch_add(1);
+  struct Release {
+    ~Release() {
+      for (b200_pair* p : held) p->host_ops.fetch_sub(1);
+    }
+  } release;
+  if (any_device_owned((const b200_pair* const*)sops, ns, sizeof(b200_send_op), "b200_pairs_submit") ||
+      any_device_owned((const b200_pair* const*)rops, nr, sizeof(b200_recv_op), "b200_pairs_submit"))
+    return -1;
   if (!r.svc_running.load()) {
     int rc = 0;
     if (ns) rc = b200_pairs_send(sops, ns, flags, accepted, nullptr);
@@ -2113,6 +2344,7 @@ struct b200_async {
   int hstage_cls = -1;
   void* dst = nullptr;
   cudaEvent_t ev = nullptr;
+  bool counted = false;  // posted: counts in p->host_ops until it is finished
 };
 
 namespace {
@@ -2143,6 +2375,8 @@ b200_async* async_get() {
   return o;
 }
 void async_put(b200_async* o) {
+  if (o->counted) o->p->host_ops.fetch_sub(1);
+  o->counted = false;
   AsyncPool& a = AP();
   std::lock_guard<std::mutex> lk(a.mu);
   if (o->stage) a.free_stage[o->stage_cls].push_back(o->stage);
@@ -2184,6 +2418,14 @@ extern "C" b200_async* b200_pair_post_send(b200_pair* p, const b200_slice* slice
     return nullptr;
   }
   b200_async* o = async_get();
+  o->p = p;
+  o->counted = true;  // a host op of p until it is polled to the end
+  p->host_ops.fetch_add(1);
+  if (p->device_owned.load()) {
+    set_err("b200_pair_post_send: the pair is device-owned (b200_pair_device_claim)");
+    async_put(o);
+    return nullptr;
+  }
   o->kind = 0;
   o->p = p;
   o->bytes = 0;
@@ -2251,6 +2493,14 @@ extern "C" b200_async* b200_pair_post_recv(b200_pair* p, void* dst, uint64_t cap
     return nullptr;
   }
   b200_async* o = async_get();
+  o->p = p;
+  o->counted = true;  // a host op of p until it is polled to the end
+  p->host_ops.fetch_add(1);
+  if (p->device_owned.load()) {
+    set_err("b200_pair_post_recv: the pair is device-owned (b200_pair_device_claim)");
+    async_put(o);
+    return nullptr;
+  }
   o->kind = 1;
   o->p = p;
   o->bytes = 0;
@@ -2258,7 +2508,7 @@ extern "C" b200_async* b200_pair_post_recv(b200_pair* p, void* dst, uint64_t cap
   o->state = 2;
   if (p->status != B200_CONNECTED || cap == 0) return o;
   drain_retire(p);
-  if (!p->remote && ((volatile PairMirror*)p->mirror)->has_message == 0) return o;
+  if (!p->remote && !peer_device_owned(p) && ((volatile PairMirror*)p->mirror)->has_message == 0) return o;
   const int kind = mem_kind3(dst);
   if (kind == 0) {
     set_err("b200_pair_post_recv: the destination must be GPU-addressable (b200_mem_alloc_host / register_host / device)");

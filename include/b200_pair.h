@@ -172,6 +172,40 @@ int b200_pair_get_state(b200_pair* p, b200_pair_state* out);
 /* Copy the pair's HBM ring image to host memory (cap >= ring capacity). */
 int b200_pair_copy_ring(b200_pair* p, void* host_dst, uint64_t cap);
 
+/* ------------------------------------------------------------ device API */
+/*
+ * Hand one end of a connection to the caller's own kernels: they drive it with the warp-collective calls of
+ * include/b200_device.cuh (b200_warp_send / b200_warp_recv / readiness) instead of b200_pair_send / recv.
+ *
+ * b200_pair_device_claim: the pair must be CONNECTED and have no host op in flight (a single call, a submit
+ * pass, a posted op) -- otherwise -1 and b200_last_error.  It drains an eagerly received frame's owed Retire,
+ * makes the service's owner warps drop their cached copy of the connection, marks the pair device-owned and
+ * fills *out (0).  While the pair is device-owned, host operations on THIS end are refused: b200_pair_send /
+ * recv return 0 (b200_pair_error says why), b200_pairs_send / recv / submit, b200_batch_prepare_* and
+ * b200_pair_post_* with this pair fail.  The readiness queries, get_state and copy_ring keep working (from the
+ * mirrors the device calls publish).  The PEER end is unaffected: it may stay host-driven, with or without the
+ * service, or be claimed as well.
+ * b200_pair_device_release: the caller guarantees that the kernels using the handle have finished.  The
+ * mirrors are re-published from the device state and host calls resume (0; -1 if the pair is not claimed).
+ * b200_pair_disconnect, b200_pair_init and b200_pool_putback on a claimed pair release the claim first.
+ */
+typedef struct b200_dev_pair {
+  void* table;     /* the connection table (PairDev rows, then the PairSeq side array) */
+  void* seq;       /* the PairSeq side array (stamped frames' counters) */
+  void* mirrors;   /* host-visible mirrors (pinned, mapped), indexed by slot */
+  int32_t slot;    /* this pair's row */
+  uint32_t wire;   /* 0 = loopback (same GPU), 1 = peer GPU over NVLink */
+  uint64_t _reserved[4];
+} b200_dev_pair;   /* POD, 64 bytes: pass it by pointer (device or pinned memory) or by value */
+int b200_pair_device_claim(b200_pair* p, b200_dev_pair* out);
+int b200_pair_device_release(b200_pair* p);
+/* 1 while the pair is device-owned */
+int b200_pair_device_owned(const b200_pair* p);
+
+#if defined(__cplusplus)
+static_assert(sizeof(b200_dev_pair) == 64, "b200_dev_pair is 64 bytes");
+#endif
+
 /* ------------------------------------------------------------------ poller */
 
 /* Poller::AddPollable / RemovePollable / Shutdown, poller.cc:12-49, poller.h:37.
