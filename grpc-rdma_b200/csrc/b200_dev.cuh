@@ -82,7 +82,8 @@ struct PairMirror {
   uint32_t partial_write;  // HasPendingWrites()
   uint32_t peer_exit;      // status_report.peer_exit seen by this pair
   uint32_t has_message;    // HasMessage()
-  uint32_t _reserved;
+  uint32_t dev_closed;     // 1 once b200_warp_disconnect closed this device-owned end (0 from Init on; the release
+                           // finishes the Disconnect on the host)
 };
 
 // One connection endpoint in HBM.  Three blocks with distinct writers:
@@ -98,7 +99,8 @@ struct __align__(128) PairDev {
   uint64_t* peer_credit; // address of the peer's credit block
   PairMirror* mirror;
   PairMirror* peer_mirror;  // loopback wire only, else nullptr
-  uint32_t status;       // b200_status as the host last set it
+  uint32_t status;       // b200_status: set by the host at Init / Connect / Disconnect, and to DISCONNECTED by
+                         // b200_warp_disconnect on a device-owned end
   uint32_t max_sge;      // frames per Send call (pair.cc:672); | kSgeCoalesce: one coalesced frame per call;
                          // | kSgeStamped: stamped frames both ways (set at Connect when both ends agree)
   int32_t peer_slot;     // loopback wire: index of the peer in this table, else -1
@@ -163,6 +165,7 @@ constexpr uint32_t kEvWritable = 0x4;
 
 constexpr uint32_t kStConnected = 2;
 constexpr uint32_t kStHalfClosed = 3;
+constexpr uint32_t kStDisconnected = 4;
 constexpr uint32_t kStError = 5;
 
 // ---- persistent service (b200_service_*): three resident kernels.

@@ -92,31 +92,7 @@ k_poll_scan(PairDev* __restrict__ pairs, const int32_t* __restrict__ slots, uint
   int32_t slot = -1;
   if (i < n) {
     slot = slots[i];
-    PairDev* P = &pairs[slot];
-    const uint32_t st = *(volatile uint32_t*)&P->status;
-    if (st == kStConnected) {
-      const uint32_t exit_flag = ld_acquire_u32(&P->credit_exit);
-      uint32_t hm;
-      uint64_t rd;
-      rx_probe(P->ring, P->cap, *(volatile uint64_t*)&P->head, *(volatile uint64_t*)&P->remain, rx_stamp(pairs, slot),
-               hm, rd);
-      const uint32_t pw = *(volatile uint32_t*)&P->partial_write;
-      if (exit_flag == 1) {
-        ev = kEvReadable;  // HalfClosed: force a read event (engine :1130-1137)
-      } else {
-        if (hm) ev |= kEvReadable;
-        if (pw) ev |= kEvWritable;
-      }
-      // On the loopback wire the kernels that land bytes / return credit refresh the mirrors themselves, in
-      // order with their own completion; a scan running beside them could only overwrite that with an older
-      // view (and b200_pair_recv / send answer "nothing to do" from the mirror without launching anything).
-      if (P->peer_slot < 0) {
-        publish_mirror_rx(P->mirror, P, hm, rd);
-        publish_mirror_tx(P->mirror, P);
-      }
-    } else if (st == kStError || st == kStHalfClosed) {
-      ev = kEvReadable;
-    }
+    ev = poll_events<true>(pairs, slot);  // (b200_warp.cuh: the readiness rule b200_warp_poll shares)
     events[i] = ev;
   }
   // warp-aggregated append to the ready set

@@ -661,6 +661,7 @@ extern "C" int b200_stream_sync(void* stream) {
 // ================================================================ pool / pair
 
 static void device_release_locked(Runtime& r, b200_pair* p);
+static void close_host_side(Runtime& r, b200_pair* p);
 
 extern "C" b200_pair* b200_pool_take(const char* id) {
   if (!ensure_init()) return nullptr;
@@ -965,16 +966,26 @@ extern "C" void b200_pair_disconnect(b200_pair* p) {
     q->mirror->credit_head = st.remote_head;
     q->mirror->peer_exit = 1;
   }
+  if (p->remote && was_connected) {  // the same 16-byte status write, over NVLink into the peer's table
+    cudaStreamSynchronize(r.stream);
+    struct {
+      uint64_t remote_head;
+      uint32_t peer_exit, pad;
+    } st = {p->mirror->moving_head, 1, 0};
+    cudaMemcpyAsync(p->remote_credit, &st, 16, cudaMemcpyDefault, r.stream);
+    cudaStreamSynchronize(r.stream);
+  }
+  uint32_t st = B200_DISCONNECTED;
+  cudaMemcpyAsync(&r.d_pairs[p->slot].status, &st, 4, cudaMemcpyHostToDevice, r.stream);
+  cudaStreamSynchronize(r.stream);
+  close_host_side(r, p);
+}
+
+// The host half of Disconnect, once the peer has been told and the row says DISCONNECTED (b200_pair_disconnect, or
+// b200_warp_disconnect on a device-owned end, whose release calls this): the wire mapping, the wire descriptor and
+// the address go.  Caller holds r.mu.
+static void close_host_side(Runtime& r, b200_pair* p) {
   if (p->remote) {
-    if (was_connected) {  // the same 16-byte status write, over NVLink into the peer's table
-      cudaStreamSynchronize(r.stream);
-      struct {
-        uint64_t remote_head;
-        uint32_t peer_exit, pad;
-      } st = {p->mirror->moving_head, 1, 0};
-      cudaMemcpyAsync(p->remote_credit, &st, 16, cudaMemcpyDefault, r.stream);
-      cudaStreamSynchronize(r.stream);
-    }
     if (!r.svc_running.load()) cudaIpcCloseMemHandle(p->remote_ring);  // (device-wide sync: skipped beside the service)
     p->remote = false;
     p->remote_ring = nullptr;
@@ -984,9 +995,6 @@ extern "C" void b200_pair_disconnect(b200_pair* p) {
     unlink(p->wire_file.c_str());
     p->wire_file.clear();
   }
-  uint32_t st = B200_DISCONNECTED;
-  cudaMemcpyAsync(&r.d_pairs[p->slot].status, &st, 4, cudaMemcpyHostToDevice, r.stream);
-  cudaStreamSynchronize(r.stream);
   if (p->self.qpn) r.by_qpn.erase(p->self.qpn);
   p->self.qpn = 0;
   p->peer_local = nullptr;
@@ -1006,6 +1014,8 @@ static void refresh_remote(const b200_pair* cp) {
 
 extern "C" enum b200_status b200_pair_status(b200_pair* p) {
   if (!p) return B200_UNINITIALIZED;
+  // a device-owned end that b200_warp_disconnect closed (the release finishes the Disconnect on the host)
+  if (p->device_owned.load() && ((volatile PairMirror*)p->mirror)->dev_closed) return B200_DISCONNECTED;
   if (p->remote && p->status == B200_CONNECTED && p->peer_pid > 0) {
     // the liveness leg of get_status (pair.cc:358-372: ibv_query_qp every 500 ms, anything but RTS -> HalfClosed).
     // On the CUDA-IPC wire there is no QP to ask: the owner process of the peer pair is probed instead -- a peer
@@ -1522,7 +1532,8 @@ static uint64_t svc_recv(Runtime& r, b200_pair* p, void* dst, uint64_t cap) {
 
 // ================================================================ device API
 
-// The host-visible mirror of p from the device state (readiness as rx_probe computes it)
+// The host-visible mirror of p from the device state (readiness as rx_probe computes it).  dev_closed is left as it
+// is: only b200_warp_disconnect sets it, Init clears it with the rest of the mirror.
 static void republish_mirror(Runtime& r, b200_pair* p) {
   PairDev hd;
   PairSeq sq;
@@ -1584,6 +1595,7 @@ extern "C" int b200_pair_device_claim(b200_pair* p, b200_dev_pair* out) {
     std::lock_guard<std::mutex> lk(r.mu);
     r.dev_slot[p->slot] = 1;
     if (r.svc_running.load()) memset((void*)&r.svc_erec[p->slot], 0, sizeof(EagerRec));  // no eager Recv any more
+    ((volatile PairMirror*)p->mirror)->dev_closed = 0;  // (a CONNECTED end: clear since Init; set only by the device)
     r.svc_gen++;
     memset(out, 0, sizeof(*out));
     out->table = r.d_pairs;
@@ -1622,6 +1634,8 @@ static void device_release_locked(Runtime& r, b200_pair* p) {
   r.dev_slot[p->slot] = 0;
   p->device_owned = false;
   if (p->error == kDeviceOwnedRefusal) p->error.clear();
+  // b200_warp_disconnect told the peer and marked the row: the rest of the Disconnect, with no second peer_exit write
+  if (p->status == B200_CONNECTED && ((volatile PairMirror*)p->mirror)->dev_closed) close_host_side(r, p);
 }
 
 extern "C" int b200_pair_device_release(b200_pair* p) {

@@ -571,4 +571,96 @@ __device__ inline uint64_t warp_readable(PairDev* table, int slot, uint32_t* has
   return rd;
 }
 
+// ======================================================================= poll, status, writable, Disconnect
+
+// The kEv* readiness of pair `slot`, by ONE lane: the per-pair body of Poller::begin_polling (poller.cc:66-101) and of
+// the engine's busy-poll window (ev_epollex_rdma_bpev_linux.cc:1104-1145).  A CONNECTED pair whose peer has left is
+// READABLE (the read that reports the close); otherwise READABLE on HasMessage, WRITABLE on HasPendingWrites.  An
+// ERROR or HALF_CLOSED row is READABLE.  Acquire loads: the ring and the credit word may be written from outside this
+// GPU.  k_poll_scan and b200_warp_poll both run this.  kPublish (k_poll_scan): also refresh the host mirror of a pair
+// off the loopback wire, whose bytes and credit nothing on this GPU publishes; a lock-free scan beside the ops of the
+// pair would overwrite a newer view with an older one, so the device API never publishes from here.
+template <bool kPublish>
+__device__ __forceinline__ uint32_t poll_events(PairDev* __restrict__ pairs, int slot) {
+  PairDev* P = &pairs[slot];
+  uint32_t ev = 0;
+  const uint32_t st = *(volatile uint32_t*)&P->status;
+  if (st == kStConnected) {
+    const uint32_t exit_flag = ld_acquire_u32(&P->credit_exit);
+    uint32_t hm;
+    uint64_t rd;
+    rx_probe(P->ring, P->cap, *(volatile uint64_t*)&P->head, *(volatile uint64_t*)&P->remain, rx_stamp(pairs, slot),
+             hm, rd);
+    const uint32_t pw = *(volatile uint32_t*)&P->partial_write;
+    if (exit_flag == 1) {
+      ev = kEvReadable;  // HalfClosed: force a read event (engine :1130-1137)
+    } else {
+      if (hm) ev |= kEvReadable;
+      if (pw) ev |= kEvWritable;
+    }
+    // On the loopback wire the kernels that land bytes / return credit refresh the mirrors themselves, in
+    // order with their own completion; a scan running beside them could only overwrite that with an older
+    // view (and b200_pair_recv / send answer "nothing to do" from the mirror without launching anything).
+    if (kPublish && P->peer_slot < 0) {
+      publish_mirror_rx(P->mirror, P, hm, rd);
+      publish_mirror_tx(P->mirror, P);
+    }
+  } else if (st == kStError || st == kStHalfClosed) {
+    ev = kEvReadable;
+  }
+  return ev;
+}
+
+// get_status (pair.cc:349-375) as far as the device can tell: the row's status, HALF_CLOSED on a CONNECTED row whose
+// peer has written peer_exit.  (Whether the peer's process still exists is a host question: b200_pair_status.)
+__device__ __forceinline__ uint32_t pair_status(PairDev* table, int slot) {
+  PairDev* P = table + slot;
+  const uint32_t st = VL(P->status);
+  return st == kStConnected && ld_acquire_u32(&P->credit_exit) == 1 ? kStHalfClosed : st;
+}
+
+// GetWritableSize (pair.cc:294-301) from the device state
+__device__ __forceinline__ uint64_t pair_writable(PairDev* table, int slot) {
+  PairDev* P = table + slot;
+  return writable_size(VL(P->cap), ld_acquire_u64(&P->credit_head), VL(P->remote_tail));
+}
+
+// PairPollable::Disconnect (pair.cc:325-347) of a device-owned end, by one warp.  Returns 0 and changes nothing on a
+// row that is not CONNECTED.  Otherwise: (1) a fence (system scope on the nvlink wire), so every frame and clear this
+// end wrote is visible before the peer can see the close; (2) unless the peer has left already, the 16-byte
+// status_report {moving_head, peer_exit = 1} into the peer's credit block -- on the loopback wire with the peer's
+// mirror, under the peer's mirror lock; (3) the row's status = DISCONNECTED, so every later call on the end refuses;
+// (4) the end's mirror flag that tells the host the rest of the Disconnect is due at the release.  Returns 1.
+__device__ inline int warp_disconnect(PairDev* table, int slot, uint32_t lane) {
+  PairDev* P = table + slot;
+  uint32_t st = 0;
+  if (lane == 0) st = VL(P->status);
+  st = __shfl_sync(0xffffffffu, st, 0);
+  if (st != kStConnected) return 0;
+  if (lane == 0) {
+    if (VL(P->wire) != 0) __threadfence_system();
+    else __threadfence();
+    if (ld_acquire_u32(&P->credit_exit) != 1) {
+      const uint64_t mh = VL(P->moving_head);
+      const int peer_slot = VL(P->peer_slot);
+      PairDev* Q = peer_slot >= 0 ? table + peer_slot : nullptr;
+      if (Q) mirror_lock(Q, true);
+      asm volatile("st.global.v2.u64 [%0], {%1,%2};" ::"l"(VL(P->peer_credit)), "l"(mh), "l"(1ull) : "memory");
+      PairMirror* pm = VL(P->peer_mirror);
+      if (pm) {
+        volatile PairMirror* vm = pm;
+        vm->credit_head = mh;
+        vm->peer_exit = 1;
+      }
+      if (Q) mirror_unlock(Q, true);
+    }
+    VL(P->status) = kStDisconnected;
+    PairMirror* m = VL(P->mirror);
+    __threadfence_system();
+    if (m) ((volatile PairMirror*)m)->dev_closed = 1;
+  }
+  __syncwarp();
+  return 1;
+}
+
 }  // namespace b200

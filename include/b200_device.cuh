@@ -12,6 +12,8 @@
  *   b200_warp_send      one PairPollable::Send call: b200_pair_send from the same state
  *   b200_warp_recv      one PairPollable::Recv call: b200_pair_recv from the same state
  *   b200_warp_readable / b200_warp_has_message / b200_warp_has_pending_writes: the readiness queries
+ *   b200_warp_poll / b200_warp_status / b200_warp_writable / b200_warp_disconnect: the Poller's scan over many ends,
+ *                       get_status, GetWritableSize and Disconnect (below)
  * They never wait: Send returns 0 when there is no credit, Recv returns 0 when no complete frame is at the head.
  * The caller decides how to retry and bounds its own loop.
  *
@@ -62,6 +64,59 @@ __device__ inline int b200_warp_has_message(const b200_dev_pair* h) {
 }
 __device__ inline int b200_warp_has_pending_writes(const b200_dev_pair* h) {
   return *(volatile const uint32_t*)&reinterpret_cast<b200::PairDev*>(h->table)[h->slot].partial_write != 0;
+}
+
+/* ---- the poll loop of a BPEV server: poll, status, writable, Disconnect (DESIGN.md §13) ---------------------------
+ *
+ * b200_warp_poll: the readiness of n claimed ends, one lane per handle, 32 handles per round (any n, 0 included).
+ * events[i] (may be NULL) gets the B200_EV_* bits b200_poller_scan gives the same pair from the same state: on a
+ * CONNECTED end READABLE when the peer has left, otherwise READABLE on HasMessage (reference format: a header word
+ * at the head counts, footer or not; stamped frames: a complete frame with the expected stamp) and WRITABLE on
+ * HasPendingWrites; READABLE on an ERROR or HALF_CLOSED end; 0 otherwise.  ready (may be NULL) gets the indices i
+ * with non-zero events in ascending order; the call returns how many there are.  It never waits, takes no lock and
+ * writes no mirror: a device-owned end publishes its own mirror under the pair's lock in its Send / Recv calls, and a
+ * lock-free scan that wrote mirrors could overwrite a newer view.  The rule is k_poll_scan's, in the same code.
+ */
+__device__ inline uint32_t b200_warp_poll(const b200_dev_pair* handles, uint32_t n, uint32_t* events,
+                                          uint32_t* ready) {
+  const uint32_t lane = b200_lane_id();
+  uint32_t count = 0;
+  for (uint32_t base = 0; base < n; base += 32) {
+    const uint32_t i = base + lane;
+    uint32_t ev = 0;
+    if (i < n) {
+      ev = b200::poll_events<false>(reinterpret_cast<b200::PairDev*>(handles[i].table), handles[i].slot);
+      if (events) events[i] = ev;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, ev != 0);
+    if (ready && ev) ready[count + __popc(m & ((1u << lane) - 1))] = i;
+    count += __popc(m);
+  }
+  __syncwarp();
+  return count;
+}
+
+/* get_status (pair.cc:349-375) from the device state: a b200_status, HALF_CLOSED on a CONNECTED end whose peer has
+ * left.  b200_pair_status also probes, every 500 ms, whether the peer's process still exists (CUDA-IPC wire): a
+ * kernel cannot ask that, so a peer process that died without Disconnect shows here only once the host has seen it. */
+__device__ inline int b200_warp_status(const b200_dev_pair* h) {
+  return (int)b200::pair_status(reinterpret_cast<b200::PairDev*>(h->table), h->slot);
+}
+
+/* GetWritableSize (pair.cc:294-301): b200_pair_writable's formula on the device's credit word and tail. */
+__device__ inline uint64_t b200_warp_writable(const b200_dev_pair* h) {
+  return b200::pair_writable(reinterpret_cast<b200::PairDev*>(h->table), h->slot);
+}
+
+/* PairPollable::Disconnect (pair.cc:325-347) from the device: 0 (nothing changed) unless the end is CONNECTED;
+ * otherwise a fence (system scope on the nvlink wire) so that everything this end wrote is visible, the peer's
+ * peer_exit = 1 with this end's moving head (as b200_pair_disconnect writes it; not when the peer has left already),
+ * the end DISCONNECTED -- every later call on it returns 0 -- and 1.  The peer sees HALF_CLOSED at once; a
+ * b200_pair_status of this end says DISCONNECTED.  b200_pair_device_release then finishes the Disconnect on the host
+ * (the wire and the address go), with no second write to the peer.  Counts as both a Send and a Recv under the
+ * ops-in-flight rule: no Send or Recv of this end may run beside it. */
+__device__ inline int b200_warp_disconnect(const b200_dev_pair* h) {
+  return b200::warp_disconnect(reinterpret_cast<b200::PairDev*>(h->table), h->slot, b200_lane_id());
 }
 
 #endif /* B200_DEVICE_CUH */

@@ -188,6 +188,10 @@ int b200_pair_copy_ring(b200_pair* p, void* host_dst, uint64_t cap);
  * b200_pair_device_release: the caller guarantees that the kernels using the handle have finished.  The
  * mirrors are re-published from the device state and host calls resume (0; -1 if the pair is not claimed).
  * b200_pair_disconnect, b200_pair_init and b200_pool_putback on a claimed pair release the claim first.
+ * An end the device closed with b200_warp_disconnect: b200_pair_status says DISCONNECTED from then on; the release
+ * finishes the Disconnect on the host (the wire and the address go, nothing more is written to the peer), after which
+ * b200_pair_init, Connect and b200_pool_putback work as after b200_pair_disconnect -- which, on such an end, is the
+ * release and nothing else.
  */
 typedef struct b200_dev_pair {
   void* table;     /* the connection table (PairDev rows, then the PairSeq side array) */
