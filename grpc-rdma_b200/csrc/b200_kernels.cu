@@ -142,6 +142,7 @@ struct ConnView {    // what an op works on
   PairSvc* SP;
   PairSvc* SQ;
   PairSeq* NP;       // the op's pair's frame counters (cached copy)
+  PairSeq* NQ;       // its loopback peer's, or nullptr
 };
 
 __device__ __forceinline__ ConnView conn_get(ConnEntry* cc, uint32_t& cc_next, const SvcParams& sp, int pslot,
@@ -200,6 +201,7 @@ __device__ __forceinline__ ConnView conn_get(ConnEntry* cc, uint32_t& cc_next, c
   const bool has_q = e.slot[side ^ 1] >= 0 && e.slot[side ^ 1] == e.line[side].peer_slot;
   v.Q = has_q ? &e.line[side ^ 1] : nullptr;
   v.SQ = has_q ? &e.svc[side ^ 1] : nullptr;
+  v.NQ = has_q ? &e.seq[side ^ 1] : nullptr;
   return v;
 }
 
@@ -343,9 +345,11 @@ __device__ __forceinline__ void svc_send_small(const SvcParams& sp, const ConnVi
   const uint64_t foff = (rt + a) & mask;
   const uint32_t st = stamped ? stamp_of(tx + lane) : 0;  // frames are lanes 0..nframes-1
   const uint64_t hdr = frame_header(p, st);
-  // eager: the first frame lands exactly at the head of the peer's (empty) ring
+  // eager: the first frame lands exactly at the head of the peer's (empty) ring.  Stamped, it is the peer's next
+  // message only if it carries the stamp the peer expects (its rx counter's), as every reader checks
   const uint64_t p0 = __shfl_sync(0xffffffffu, p, 0);
-  const bool at_head = peer_slot >= 0 && nframes > 0 && cv.Q->remain == 0 && cv.Q->head == rt;
+  const bool at_head = peer_slot >= 0 && nframes > 0 && cv.Q->remain == 0 && cv.Q->head == rt &&
+                       (!stamped || stamp_of(cv.NQ->rx) == stamp_of(tx));
   const bool eager = at_head && p0 <= kEagerMax && sp.erec != nullptr && cv.SQ->pushed_at != cv.SQ->delivered;
   uint8_t* eslot = eager ? sp.eslots + (size_t)peer_slot * kEagerMax : nullptr;
   const uint64_t cs = send_frames(ring, mask, ptr, p, foff, hdr, nframes, eslot, lane);
@@ -434,7 +438,8 @@ __device__ __forceinline__ void svc_send_small_coalesced(const SvcParams& sp, co
   const uint64_t pmax = ws < wf ? ws : wf;
   uint64_t p = __shfl_sync(0xffffffffu, incl, 7);
   if (p > pmax) p = pmax;
-  const bool at_head = peer_slot >= 0 && p > 0 && cv.Q->remain == 0 && cv.Q->head == rt;
+  const bool at_head = peer_slot >= 0 && p > 0 && cv.Q->remain == 0 && cv.Q->head == rt &&
+                       (!stamped || stamp_of(cv.NQ->rx) == st);
   const bool eager = at_head && p <= kEagerMax && sp.erec != nullptr && cv.SQ->pushed_at != cv.SQ->delivered;
   uint8_t* eslot = eager ? sp.eslots + (size_t)peer_slot * kEagerMax : nullptr;
   uint64_t cs = 0;
