@@ -288,8 +288,11 @@ uint64_t b200_service_eager_hits(void);
  *                        connection always maps to the same lane, which keeps its Send and Recv
  *                        ordered.  With a NULL stream the lanes run free (b200_lanes_join or
  *                        b200_batch_results to wait); with a stream the batch forks from / joins
- *                        back into it.  B200_BATCH_ZEROCOPY instead lets the kernels read and
- *                        write the pinned buffers directly (GPUDirect-style, no staging).
+ *                        back into it.  A Recv copies its WHOLE destination window back: bytes
+ *                        past `delivered` are the batch's staging bytes there (zero, or what an
+ *                        earlier launch of the same batch delivered).  B200_BATCH_ZEROCOPY
+ *                        instead lets the kernels read and write the pinned buffers directly
+ *                        (GPUDirect-style, no staging).
  */
 
 /* Threading of this section: a prepared batch belongs to one thread at a time (launch / results / destroy are not
