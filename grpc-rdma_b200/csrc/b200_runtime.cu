@@ -262,6 +262,9 @@ struct Runtime {
   // B200_BATCH_CONCURRENT, so the owner warp reads that connection's lines fresh and publishes its mirrors under the
   // per-pair locks (a user kernel changes them meanwhile)
   std::atomic<uint8_t> dev_slot[kMaxPairs] = {};
+  // ops of launched prepared batches whose results have not been collected, per slot: a command for a connection
+  // with such an op carries B200_BATCH_CONCURRENT as well (the batch's kernels change its lines meanwhile)
+  std::atomic<uint16_t> batch_slot[kMaxPairs] = {};
   uint32_t svc_ready_head = 0;      // next stream index the host expects (under scan_mu)
   std::vector<uint16_t> svc_level;  // events pending per slot, as last reported by the device poller
   std::mutex grave_mu;
@@ -1206,7 +1209,8 @@ static bool svc_try_post(Runtime& r, int q, Fill fill, uint64_t* ticket) {
   c->nreal = 0;
   fill(c, r.svc_slices + e * (kSvcSliceArea + 1));
   const int s0 = c->slot & 0xffff, s1 = (c->slot >> 16) - 1;
-  if ((s0 < kMaxPairs && r.dev_slot[s0].load()) || (s1 >= 0 && s1 < kMaxPairs && r.dev_slot[s1].load()))
+  if ((s0 < kMaxPairs && (r.dev_slot[s0].load() || r.batch_slot[s0].load())) ||
+      (s1 >= 0 && s1 < kMaxPairs && (r.dev_slot[s1].load() || r.batch_slot[s1].load())))
     c->flags |= B200_BATCH_CONCURRENT;
   c->op = (c->op & 0xffu) | ((r.svc_gen.load(std::memory_order_acquire) & 0xffffffu) << 8);
   std::atomic_thread_fence(std::memory_order_release);
@@ -2044,9 +2048,10 @@ extern "C" int b200_lanes_join(void* stream) {
   return 0;
 }
 
-// a device-owned peer publishes its mirror fields under the per-pair locks: so must the batch's kernels
+// a device-owned peer, and the service's owner warps, publish mirror fields under the per-pair locks: so must the
+// batch's kernels
 static bool batch_make_concurrent(b200_batch* b) {
-  bool need = false;
+  bool need = R().svc_running.load();
   for (const b200_pair* p : b->op_pairs) need = need || (p->peer_local && p->peer_local->device_owned.load());
   if (!need || (b->flags & B200_BATCH_CONCURRENT)) return true;
   b->flags |= B200_BATCH_CONCURRENT;
@@ -2059,7 +2064,14 @@ static bool batch_make_concurrent(b200_batch* b) {
 }
 static void batch_uncount(b200_batch* b) {
   if (!b->counted) return;
-  for (b200_pair* p : b->op_pairs) p->host_ops.fetch_sub(1);
+  Runtime& r = R();
+  // the kernels have changed the pairs' lines behind the owners' caches: a new generation first, so that a command
+  // that no longer sees the batch's ops in batch_slot carries it
+  if (r.svc_running.load()) r.svc_gen++;
+  for (b200_pair* p : b->op_pairs) {
+    r.batch_slot[p->slot].fetch_sub(1);
+    p->host_ops.fetch_sub(1);
+  }
   b->counted = false;
 }
 
@@ -2070,7 +2082,10 @@ extern "C" int b200_batch_launch(b200_batch* b, void* stream) {
   // from here until its results are collected the batch is a host op of each of its pairs (counted first, then the
   // ownership looked at: see HostOp)
   if (!b->counted) {
-    for (b200_pair* p : b->op_pairs) p->host_ops.fetch_add(1);
+    for (b200_pair* p : b->op_pairs) {
+      p->host_ops.fetch_add(1);
+      r.batch_slot[p->slot].fetch_add(1);
+    }
     b->counted = true;
   }
   if (any_device_owned((const b200_pair* const*)b->op_pairs.data(), b->op_pairs.size(), sizeof(b200_pair*),

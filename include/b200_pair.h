@@ -298,7 +298,16 @@ uint64_t b200_service_eager_hits(void);
 /* Threading of this section: a prepared batch belongs to one thread at a time (launch / results / destroy are not
  * locked against each other); different batches may be driven from different threads, the host-staged lanes and the
  * runtime's default stream are shared, so concurrent launches interleave there in submission order.
- * b200_pairs_submit and the post / poll calls are thread-safe (per-queue posting sections, per-thread staging). */
+ * b200_pairs_submit and the post / poll calls are thread-safe (per-queue posting sections, per-thread staging).
+ *
+ * A batch launched while the service runs (b200_service_start) may run beside single calls on the same connection,
+ * within the rule above: one Send and one Recv of a pair at a time, e.g. a batch Send on one end and b200_pair_recv on
+ * the other.  From the launch until b200_batch_results (or b200_batch_destroy), the service reads that connection's
+ * state fresh for every call and publishes both ends' readiness under the per-pair locks, as the batch's kernels do
+ * (B200_BATCH_CONCURRENT is implied); once the results are collected, no call works from a view taken before the
+ * batch ran.  A single call that returns before the batch runs is ordered before it, one that starts after
+ * b200_batch_results is ordered after it; in between, the per-op counts depend on timing and the byte stream does
+ * not. */
 typedef struct b200_send_op {
   b200_pair* pair;
   const b200_slice* slices; /* host array of n entries (copied at submit) */
