@@ -1,5 +1,6 @@
 /*
- * b200_device_block.cuh -- block-level device Send / Recv on a pair, for user kernels (sm_90a).
+ * b200_device_block.cuh -- block-level device Send / Recv on a pair, for user kernels (sm_90a), and their cluster form
+ * (b200_cluster_send / b200_cluster_recv, below).
  *
  * The warp calls of b200_device.cuh move a connection's bytes with one warp and plain loads and stores.  The calls
  * here put a whole CTA on the op and run the library's own k_send / k_recv pipeline on it: warp 0 plans the frames,
@@ -59,6 +60,7 @@ typedef struct b200_block {
   b200::OpResult res;                   // the op's answer, broadcast to every thread
   uint32_t go;                          // the entry checks' answer
   uint32_t phase[1 + b200::kMovers];    // per warp: the parities of its stage barriers, carried from op to op
+  b200::PairDev* table;                 // cluster calls: the connection table of the op (rank 0's handle)
 } b200_block;
 
 // The movers' stages: the first B200_BLOCK_SMEM_BYTES of the kernel's dynamic shared memory.  They are addressed from
@@ -143,6 +145,119 @@ __device__ inline uint64_t b200_block_recv(b200_block* st, const b200_dev_pair* 
   uint32_t phase = st->phase[threadIdx.x >> 5];
   b200::recv_body(table, st->rop, &st->res, st->pipe, b200_block_stages, phase);
   return b200_block_leave(st, phase, calls);
+}
+
+/* ---- cluster calls: a thread-block cluster of K CTAs drives one op ------------------------------------------------
+ *
+ * One CTA keeps at most 8 movers x 3 stages x 4 KiB of reads in flight, far below what HBM needs to run near its rate;
+ * with few connections most of the GPU would sit idle.  b200_cluster_send / b200_cluster_recv run one op on a cluster:
+ * the planner warp of CTA rank 0 plans it as the block calls do, and the mover warps of all K CTAs move its 4 KiB items,
+ * item i in CTA i mod K, each CTA with its own stages and bulk-copy engine (DESIGN.md §13, "Cluster calls").
+ *
+ * Every call is CLUSTER-COLLECTIVE: every thread of every CTA of the cluster calls it.  The op is taken from the
+ * arguments of CTA rank 0 (the other CTAs' arguments are ignored) and every thread gets the same result, with the
+ * semantics of b200_block_send / b200_block_recv: return values, *calls, partial_write, cursors, credit, frames and
+ * ring image bit for bit, in every framing mode.
+ *
+ * Rules, beyond those of the block calls (the CTA shape, __launch_bounds__(B200_BLOCK_THREADS, 2), the stages, one
+ * b200_block per CTA with b200_block_init, the memory of slices and dst, the claim):
+ *   - the cluster is K x 1 x 1 CTAs, 1 <= K <= 16 (K is read from %cluster_nctarank; K > 8 needs
+ *     cudaFuncAttributeNonPortableClusterSizeAllowed on the kernel).  K = 1, a launch without clusters, runs the
+ *     block calls' pipeline on the one CTA, with the same results;
+ *   - at most one sending cluster, CTA or warp and one receiving cluster, CTA or warp per pair at a time;
+ *   - the calls never wait; clusters that wait for each other must be co-resident (cudaOccupancyMaxActiveClusters);
+ *   - when b200_cluster_recv returns, the delivered bytes are visible to every thread of the cluster.  Rank 0
+ *     publishes the mirrors under the per-pair lock, once per op.
+ * Refusals return 0 (and *calls = 0) to every thread and change nothing: those of the block calls, and a cluster that
+ * is not K x 1 x 1 with K <= 16.
+ */
+__device__ __forceinline__ bool b200_cluster_shape_ok() {
+  uint32_t y, z;
+  asm volatile("mov.u32 %0, %%cluster_nctaid.y;" : "=r"(y));
+  asm volatile("mov.u32 %0, %%cluster_nctaid.z;" : "=r"(z));
+  return y == 1 && z == 1 && b200::cluster_nctarank() <= 16;
+}
+
+// Thread 0 of rank 0 has written the op, its table and the entry checks' answer into its b200_block; after the cluster
+// barrier every other CTA copies them into its own.  A refused op returns only after a second cluster barrier, so that
+// rank 0 cannot overwrite them with the next call's before every CTA has read them.
+template <class Op>
+__device__ __forceinline__ bool b200_cluster_enter(b200_block* st, Op* op) {
+  static_assert(sizeof(Op) % 8 == 0, "the op is copied in 8-byte words");
+  constexpr uint32_t kWords = sizeof(Op) / 8;
+  b200::cluster_sync();
+  if (b200::cluster_ctarank() != 0) {
+    const uint32_t t = threadIdx.x;
+    uint64_t* w = reinterpret_cast<uint64_t*>(op);
+    if (t < kWords) w[t] = b200::cl_ld_u64(b200::cl_map(w + t, 0));
+    else if (t == kWords) st->table = reinterpret_cast<b200::PairDev*>(b200::cl_ld_u64(b200::cl_map(&st->table, 0)));
+    else if (t == kWords + 1) st->go = b200::cl_ld_u32(b200::cl_map(&st->go, 0));
+  }
+  __syncthreads();
+  if (st->go) return true;
+  b200::cluster_sync();
+  return false;
+}
+
+// The end of every op that ran: this warp's stage parities, then rank 0's answer to every thread of the cluster.  The
+// second barrier keeps every CTA in the call (and rank 0's shared memory alive) until every CTA has read the answer.
+__device__ __forceinline__ uint64_t b200_cluster_leave(b200_block* st, uint32_t phase, uint64_t* calls) {
+  if ((threadIdx.x & 31) == 0) st->phase[threadIdx.x >> 5] = phase;
+  b200::cluster_sync();
+  const uint32_t a = b200::cl_map(&st->res, 0);
+  const uint64_t bytes = b200::cl_ld_u64(a + offsetof(b200::OpResult, bytes));
+  const uint64_t c = b200::cl_ld_u64(a + offsetof(b200::OpResult, calls));
+  b200::cluster_sync();
+  if (calls) *calls = c;
+  return bytes;
+}
+
+/* Cluster-collective b200_block_send: payload bytes accepted; *calls (may be NULL) = Send calls that accepted bytes. */
+__device__ inline uint64_t b200_cluster_send(b200_block* st, const b200_dev_pair* h, const b200_slice* slices,
+                                             uint64_t n, uint64_t byte_idx, int flags, uint64_t* calls) {
+  if (calls) *calls = 0;
+  if (!b200_block_shape_ok() || !b200_cluster_shape_ok()) return 0;
+  if (threadIdx.x == 0 && b200::cluster_ctarank() == 0) {
+    b200::PairDev* table = reinterpret_cast<b200::PairDev*>(h->table);
+    const b200::PairDev* P = table + h->slot;
+    st->go = (flags & ~B200_BATCH_UNTIL_BLOCKED) == 0 && *(volatile const uint32_t*)&P->status == b200::kStConnected &&
+             n != 0 && b200::ld_acquire_u32(&P->credit_exit) != 1;
+    st->table = table;
+    b200::SendOpDev& op = st->sop;
+    op.slot = h->slot;
+    op.flags = (uint32_t)flags | b200::kFlagConcurrent;
+    op.slices = reinterpret_cast<const b200::SliceDev*>(slices);
+    op.nslices = n;
+    op.byte_idx = byte_idx;
+    op.nreal = n;
+  }
+  if (!b200_cluster_enter(st, &st->sop)) return 0;
+  uint32_t phase = st->phase[threadIdx.x >> 5];
+  b200::send_body<true>(st->table, st->sop, &st->res, st->pipe, b200_block_stages, phase);
+  return b200_cluster_leave(st, phase, calls);
+}
+
+/* Cluster-collective b200_block_recv: bytes delivered into dst; *calls (may be NULL) = Recv calls that delivered
+ * bytes. */
+__device__ inline uint64_t b200_cluster_recv(b200_block* st, const b200_dev_pair* h, void* dst, uint64_t cap, int flags,
+                                             uint64_t* calls) {
+  if (calls) *calls = 0;
+  if (!b200_block_shape_ok() || !b200_cluster_shape_ok()) return 0;
+  if (threadIdx.x == 0 && b200::cluster_ctarank() == 0) {
+    b200::PairDev* table = reinterpret_cast<b200::PairDev*>(h->table);
+    st->go = (flags & ~B200_BATCH_UNTIL_BLOCKED) == 0 &&
+             *(volatile const uint32_t*)&table[h->slot].status == b200::kStConnected && cap != 0;
+    st->table = table;
+    b200::RecvOpDev& op = st->rop;
+    op.slot = h->slot;
+    op.flags = (uint32_t)flags | b200::kFlagConcurrent;
+    op.dst = static_cast<uint8_t*>(dst);
+    op.cap = cap;
+  }
+  if (!b200_cluster_enter(st, &st->rop)) return 0;
+  uint32_t phase = st->phase[threadIdx.x >> 5];
+  b200::recv_body<true>(st->table, st->rop, &st->res, st->pipe, b200_block_stages, phase);
+  return b200_cluster_leave(st, phase, calls);
 }
 
 #endif /* B200_DEVICE_BLOCK_CUH */
