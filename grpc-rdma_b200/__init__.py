@@ -12,6 +12,7 @@ The directory name contains a hyphen, so load it with
 ``__graft_entry__.load_package()`` (registers it as ``grpc_rdma_b200``).
 """
 import ctypes as C
+import numbers
 import os
 import subprocess
 
@@ -27,6 +28,14 @@ DEV_PAIR_BYTES = 64  # sizeof(b200_dev_pair)
 ONE_CALL, UNTIL_BLOCKED, ASYNC, ZEROCOPY = 0, 1, 2, 4
 EV_READABLE, EV_WRITABLE = 0x1, 0x4
 STATUS = ["UNINITIALIZED", "INITIALIZED", "CONNECTED", "HALF_CLOSED", "DISCONNECTED", "ERROR"]
+
+
+def cluster_flag(k):
+    """B200_BATCH_CLUSTER(k): batch flag bits that run each op on a thread-block cluster of k CTAs (1 <= k <= 16;
+    k = 1 is the default, one CTA per op)."""
+    if isinstance(k, bool) or not isinstance(k, numbers.Integral) or not 1 <= k <= 16:
+        raise ValueError("cluster width must be an integer in 1..16, got %r" % (k,))
+    return (int(k) - 1) << 4
 
 
 class Slice(C.Structure):

@@ -271,8 +271,12 @@ struct SvcParams {
 };
 
 // launch wrappers (b200_kernels.cu)
-void launch_send(PairDev* pairs, const SendOpDev* ops, OpResult* results, int nops, void* stream);
-void launch_recv(PairDev* pairs, const RecvOpDev* ops, OpResult* results, int nops, void* stream);
+// cluster >= 2 (B200_BATCH_CLUSTER): each op runs on a cluster of that many CTAs (k_cluster_send / k_cluster_recv)
+void launch_send(PairDev* pairs, const SendOpDev* ops, OpResult* results, int nops, void* stream, int cluster = 1);
+void launch_recv(PairDev* pairs, const RecvOpDev* ops, OpResult* results, int nops, void* stream, int cluster = 1);
+// clusters of `cluster` CTAs of k_cluster_send (kind 0) / k_cluster_recv (kind 1) the device can hold at once, with
+// nothing else resident (cudaOccupancyMaxActiveClusters); 0: it cannot place one
+int cluster_capacity(int kind, int cluster);
 void launch_poll_scan(PairDev* pairs, const int32_t* slots, uint32_t* events, uint32_t* ready_count,
                       int32_t* ready_slots, int n, void* stream);
 

@@ -80,6 +80,52 @@ k_recv(PairDev* __restrict__ pairs, const RecvOpDev* __restrict__ ops, OpResult*
 }
 
 // =========================================================================
+// k_cluster_send / k_cluster_recv: batches launched with B200_BATCH_CLUSTER(K), K >= 2
+// =========================================================================
+//
+// One op per thread-block cluster of K CTAs (op = cluster index): every CTA runs the cluster form of the body on it,
+// rank 0 plans and writes the answer, the movers of all K CTAs move its items (DESIGN.md §13).  The body's first
+// cluster barrier comes before any access to another CTA's shared memory.  Each kernel ends on a cluster barrier on
+// every path -- the body returns without one for a pair that is not connected -- so that no CTA leaves while another
+// may still read its shared memory.
+
+__global__ void __launch_bounds__(kThreads, 2)
+k_cluster_send(PairDev* __restrict__ pairs, const SendOpDev* __restrict__ ops, OpResult* __restrict__ results) {
+  extern __shared__ __align__(128) uint8_t stage_mem[];
+  __shared__ PipeSmem pipe;
+  movers_init(pipe, threadIdx.x);
+  uint32_t phase_bits = 0;
+  const uint32_t o = blockIdx.x / cluster_nctarank();
+  const SendOpDev op = ops[o];
+  send_body<true>(pairs, op, &results[o], pipe, stage_mem, phase_bits);
+  cluster_sync();
+}
+
+// The op and the table pointer are read from shared memory, as the cluster calls hold them in b200_block: with the
+// op in registers, as k_recv takes it, this kernel spills 12 bytes.
+struct RecvClArgs {
+  RecvOpDev op;
+  PairDev* table;
+};
+
+__global__ void __launch_bounds__(kThreads, 2)
+k_cluster_recv(PairDev* __restrict__ pairs, const RecvOpDev* __restrict__ ops, OpResult* __restrict__ results) {
+  extern __shared__ __align__(128) uint8_t stage_mem[];
+  __shared__ PipeSmem pipe;
+  __shared__ RecvClArgs args;
+  movers_init(pipe, threadIdx.x);
+  uint32_t phase_bits = 0;
+  const uint32_t o = blockIdx.x / cluster_nctarank();
+  if (threadIdx.x == 0) {
+    args.op = ops[o];
+    args.table = pairs;
+  }
+  __syncthreads();
+  recv_body<true>(args.table, args.op, &results[o], pipe, stage_mem, phase_bits);
+  cluster_sync();
+}
+
+// =========================================================================
 // k_poll_scan
 // =========================================================================
 
@@ -1012,6 +1058,11 @@ static void ensure_kernel_attrs() {
   cudaFuncSetAttribute(k_probe_copy, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
   cudaFuncSetAttribute(k_svc_big, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStageTotal);
   cudaFuncSetAttribute(k_svc_big, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+  for (const void* f : {(const void*)k_cluster_send, (const void*)k_cluster_recv}) {
+    cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStageTotal);
+    cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    cudaFuncSetAttribute(f, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);  // clusters of 9..16 CTAs
+  }
   // Load every kernel of the library now.  With lazy module loading the first launch of a kernel loads it,
   // and a load may wait for the device to go idle: beside a resident kernel that never happens.
   cudaFuncAttributes fa;
@@ -1022,6 +1073,8 @@ static void ensure_kernel_attrs() {
   cudaFuncGetAttributes(&fa, k_svc_owner);
   cudaFuncGetAttributes(&fa, k_svc_big);
   cudaFuncGetAttributes(&fa, k_svc_poll);
+  cudaFuncGetAttributes(&fa, k_cluster_send);
+  cudaFuncGetAttributes(&fa, k_cluster_recv);
   });
 }
 
@@ -1060,15 +1113,56 @@ void launch_probe_copy(uint8_t* dst, const uint8_t* src, uint64_t bytes_per_cta,
 
 // ---------------------------------------------------------------- launchers
 
-void launch_send(PairDev* pairs, const SendOpDev* ops, OpResult* results, int nops, void* stream) {
-  if (nops <= 0) return;
-  ensure_kernel_attrs();
-  k_send<<<nops, kThreads, kStageTotal, static_cast<cudaStream_t>(stream)>>>(pairs, ops, results);
+// nops clusters of `cluster` CTAs
+static cudaLaunchConfig_t cluster_config(int nops, int cluster, void* stream, cudaLaunchAttribute* attr) {
+  cudaLaunchConfig_t c = {};
+  c.gridDim = dim3((unsigned)nops * (unsigned)cluster);
+  c.blockDim = dim3(kThreads);
+  c.dynamicSmemBytes = kStageTotal;
+  c.stream = static_cast<cudaStream_t>(stream);
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = (unsigned)cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  c.attrs = attr;
+  c.numAttrs = 1;
+  return c;
 }
-void launch_recv(PairDev* pairs, const RecvOpDev* ops, OpResult* results, int nops, void* stream) {
+
+void launch_send(PairDev* pairs, const SendOpDev* ops, OpResult* results, int nops, void* stream, int cluster) {
   if (nops <= 0) return;
   ensure_kernel_attrs();
-  k_recv<<<nops, kThreads, kStageTotal, static_cast<cudaStream_t>(stream)>>>(pairs, ops, results);
+  if (cluster <= 1) {
+    k_send<<<nops, kThreads, kStageTotal, static_cast<cudaStream_t>(stream)>>>(pairs, ops, results);
+    return;
+  }
+  cudaLaunchAttribute attr[1];
+  const cudaLaunchConfig_t c = cluster_config(nops, cluster, stream, attr);
+  cudaLaunchKernelEx(&c, k_cluster_send, pairs, ops, results);
+}
+void launch_recv(PairDev* pairs, const RecvOpDev* ops, OpResult* results, int nops, void* stream, int cluster) {
+  if (nops <= 0) return;
+  ensure_kernel_attrs();
+  if (cluster <= 1) {
+    k_recv<<<nops, kThreads, kStageTotal, static_cast<cudaStream_t>(stream)>>>(pairs, ops, results);
+    return;
+  }
+  cudaLaunchAttribute attr[1];
+  const cudaLaunchConfig_t c = cluster_config(nops, cluster, stream, attr);
+  cudaLaunchKernelEx(&c, k_cluster_recv, pairs, ops, results);
+}
+int cluster_capacity(int kind, int cluster) {
+  ensure_kernel_attrs();
+  cudaLaunchAttribute attr[1];
+  const cudaLaunchConfig_t c = cluster_config(1, cluster, nullptr, attr);
+  int n = 0;
+  const cudaError_t e = kind == 0 ? cudaOccupancyMaxActiveClusters(&n, k_cluster_send, &c)
+                                  : cudaOccupancyMaxActiveClusters(&n, k_cluster_recv, &c);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  return n;
 }
 void launch_poll_scan(PairDev* pairs, const int32_t* slots, uint32_t* events, uint32_t* ready_count,
                       int32_t* ready_slots, int n, void* stream) {

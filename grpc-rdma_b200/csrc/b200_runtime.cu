@@ -170,6 +170,7 @@ struct b200_batch {
   // host-staged path: slices / destinations are pinned HOST memory; the batch owns a device
   // staging arena and runs as kLanes independent H2D -> kernel (-> D2H) pipelines
   bool staged = false;
+  int cluster = 1;  // CTAs per op (B200_BATCH_CLUSTER): >= 2 launches k_cluster_send / k_cluster_recv
   uint8_t* d_stage = nullptr;
   std::vector<int> perm;  // perm[k] = caller's index of device op k
   std::vector<b200_pair*> pairs;  // the pairs of a Recv batch (service: their eager records go stale at launch)
@@ -1867,8 +1868,26 @@ static void push_h2d(std::vector<CopyRun>& out, uint8_t* stage, const uint8_t* s
   out.push_back({stage - lead, src - lead, lead + bytes});
 }
 
+// the cluster width of a batch's flags (B200_BATCH_CLUSTER; field 0 = 1)
+static int cluster_of(int flags) { return (int)(((unsigned)flags >> 4) & 15u) + 1; }
+constexpr int kClusterField = 0xf0;
+
+// Can this device place one cluster of `k` CTAs of the batch kernel at all?  Asked once per kind and k.
+static bool cluster_placeable(int kind, int k) {
+  static std::atomic<int> known[2][17];  // 0 = not asked yet, 1 = no, 2 = yes
+  std::atomic<int>& a = known[kind][k];
+  if (a.load() == 0) a.store(cluster_capacity(kind, k) > 0 ? 2 : 1);
+  return a.load() == 2;
+}
+
 static b200_batch* prepare_common(int kind, const void* ops_v, size_t nops, int flags) {
   if (!ensure_init()) return nullptr;
+  const int cluster = cluster_of(flags);
+  if (cluster > 1 && !cluster_placeable(kind, cluster)) {
+    set_err("b200_batch_prepare: this device cannot place a cluster of " + std::to_string(cluster) + " CTAs of the " +
+            (kind == 0 ? "Send" : "Recv") + " kernel (B200_BATCH_CLUSTER)");
+    return nullptr;
+  }
   if (any_device_owned((const b200_pair* const*)ops_v, nops, kind == 0 ? sizeof(b200_send_op) : sizeof(b200_recv_op),
                        "b200_batch_prepare"))
     return nullptr;
@@ -1878,6 +1897,7 @@ static b200_batch* prepare_common(int kind, const void* ops_v, size_t nops, int 
   b->kind = kind;
   b->nops = (int)nops;
   b->flags = flags;
+  b->cluster = cluster;
   const b200_send_op* sops = (const b200_send_op*)ops_v;
   const b200_recv_op* rops = (const b200_recv_op*)ops_v;
   bool ok = true;
@@ -2106,8 +2126,8 @@ extern "C" int b200_batch_launch(b200_batch* b, void* stream) {
   }
   if (!b->staged) {
     cudaStream_t s = stream ? (cudaStream_t)stream : r.stream;
-    if (b->kind == 0) launch_send(r.d_pairs, (const SendOpDev*)b->d_ops, b->d_results, b->nops, s);
-    else launch_recv(r.d_pairs, (const RecvOpDev*)b->d_ops, b->d_results, b->nops, s);
+    if (b->kind == 0) launch_send(r.d_pairs, (const SendOpDev*)b->d_ops, b->d_results, b->nops, s, b->cluster);
+    else launch_recv(r.d_pairs, (const RecvOpDev*)b->d_ops, b->d_results, b->nops, s, b->cluster);
     r.launches++;
     return CU_OK(cudaGetLastError()) ? 0 : -1;
   }
@@ -2125,12 +2145,14 @@ extern "C" int b200_batch_launch(b200_batch* b, void* stream) {
       for (const CopyRun& c : lp.copies)
         if (!CU_OK(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyHostToDevice, s))) return -1;
       if (!CU_OK(cudaStreamWaitEvent(s, r.recv_done[L], 0))) return -1;
-      launch_send(r.d_pairs, (const SendOpDev*)b->d_ops + lp.first_op, b->d_results + lp.first_op, lp.nops, s);
+      launch_send(r.d_pairs, (const SendOpDev*)b->d_ops + lp.first_op, b->d_results + lp.first_op, lp.nops, s,
+                  b->cluster);
       if (!CU_OK(cudaEventRecord(r.send_done[L], s))) return -1;
     } else {
       cudaStream_t s = r.lane_down[L];
       if (!CU_OK(cudaStreamWaitEvent(s, r.send_done[L], 0))) return -1;
-      launch_recv(r.d_pairs, (const RecvOpDev*)b->d_ops + lp.first_op, b->d_results + lp.first_op, lp.nops, s);
+      launch_recv(r.d_pairs, (const RecvOpDev*)b->d_ops + lp.first_op, b->d_results + lp.first_op, lp.nops, s,
+                  b->cluster);
       if (!CU_OK(cudaEventRecord(r.recv_done[L], s))) return -1;
       for (const CopyRun& c : lp.copies)
         if (!CU_OK(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, s))) return -1;
@@ -2204,6 +2226,11 @@ extern "C" int b200_pairs_recv(const b200_recv_op* ops, size_t nops, int flags, 
 extern "C" int b200_pairs_submit(const b200_send_op* sops, size_t ns, uint64_t* accepted, const b200_recv_op* rops,
                                  size_t nr, uint64_t* delivered, int flags) {
   if (!ensure_init()) return -1;
+  if (flags & kClusterField) {
+    set_err("b200_pairs_submit: B200_BATCH_CLUSTER applies to batch launches only; the service's owners and pool run "
+            "one CTA per op");
+    return -1;
+  }
   Runtime& r = R();
   // the pass counts as a host op of each of its pairs until it returns
   static thread_local std::vector<b200_pair*> held;
@@ -2446,6 +2473,11 @@ extern "C" b200_async* b200_pair_post_send(b200_pair* p, const b200_slice* slice
     set_err("b200_pair_post_send: the service is not running");
     return nullptr;
   }
+  if (flags & kClusterField) {
+    set_err("b200_pair_post_send: B200_BATCH_CLUSTER applies to batch launches only; the service's owners and pool run "
+            "one CTA per op");
+    return nullptr;
+  }
   b200_async* o = async_get();
   o->p = p;
   o->counted = true;  // a host op of p until it is polled to the end
@@ -2519,6 +2551,11 @@ extern "C" b200_async* b200_pair_post_recv(b200_pair* p, void* dst, uint64_t cap
   Runtime& r = R();
   if (!p || !r.svc_running.load()) {
     set_err("b200_pair_post_recv: the service is not running");
+    return nullptr;
+  }
+  if (flags & kClusterField) {
+    set_err("b200_pair_post_recv: B200_BATCH_CLUSTER applies to batch launches only; the service's owners and pool run "
+            "one CTA per op");
     return nullptr;
   }
   b200_async* o = async_get();

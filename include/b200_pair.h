@@ -279,6 +279,23 @@ uint64_t b200_service_eager_hits(void);
  * The service kernel always works this way; the library's own lanes order the two ends by events and
  * do not need it. */
 #define B200_BATCH_CONCURRENT 0x8
+/* Cluster width of a batch, 1 <= k <= 16, in bits 4..7 of the flags (they hold k - 1).  Field 0, the default and
+ * B200_BATCH_CLUSTER(1), is one CTA per op.  k >= 2 runs each op on a thread-block cluster of k CTAs (kernels
+ * k_cluster_send / k_cluster_recv, DESIGN.md §13): the planner of CTA rank 0 plans the op and the movers of all k
+ * CTAs move its bytes, so one connection keeps up to k times as many reads in flight.  The results are those of the
+ * same batch launched with field 0 from the same state, bit for bit -- per-op bytes and b200_batch_calls,
+ * partial_write, cursors, credit, frames and ring images, the delivered bytes and (host-staged) the whole copied-back
+ * window -- in every framing mode.  Accepted by b200_pairs_send / recv and b200_batch_prepare_send / recv on all three
+ * memory paths (device, host-staged lanes, B200_BATCH_ZEROCOPY); bits above 7 are ignored.
+ *   - The caller chooses k: whether clusters pay depends on the message size and on what else occupies the GPU.  With
+ *     few connections and large messages they do; with 64 connections on an H100, clusters of 4 or more CTAs lose.
+ *   - b200_batch_prepare_* and b200_pairs_send / recv fail (NULL / -1, b200_last_error) when
+ *     cudaOccupancyMaxActiveClusters says the device cannot place one cluster of k CTAs of the kernel.  That query
+ *     does not see resident kernels: beside the service or a user's device-API kernel, a cluster launch needs k free
+ *     CTA slots within one GPC and waits for them, as a one-CTA launch waits for one free slot.
+ *   - b200_pairs_submit and b200_pair_post_send / recv run on the service's owners and pool, not on these kernels:
+ *     they refuse a nonzero field (-1; NULL with *again = 0) and say why in b200_last_error. */
+#define B200_BATCH_CLUSTER(k) (((unsigned)(k) - 1u) << 4)
 /*
  * Where the bytes live decides the path of a batch:
  *   device memory        kernels work in place (one launch per batch);
