@@ -25,6 +25,7 @@ ENDPOINT_HEADER = os.path.join(ROOT, "include", "b200_endpoint.h")
 
 ADDRESS_BYTES = 48
 DEV_PAIR_BYTES = 64  # sizeof(b200_dev_pair)
+CLAIM_UNMIRRORED = 0x1  # B200_CLAIM_UNMIRRORED (b200_pair_device_claim_ex)
 ONE_CALL, UNTIL_BLOCKED, ASYNC, ZEROCOPY = 0, 1, 2, 4
 EV_READABLE, EV_WRITABLE = 0x1, 0x4
 STATUS = ["UNINITIALIZED", "INITIALIZED", "CONNECTED", "HALF_CLOSED", "DISCONNECTED", "ERROR"]
@@ -132,6 +133,7 @@ _SIGS = {
                                   C.c_uint32, C.c_uint32, C.c_void_p]),
     "b200_launch_count": (C.c_uint64, []),
     "b200_pair_device_claim": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "b200_pair_device_claim_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "b200_pair_device_release": (C.c_int, [C.c_void_p]),
     "b200_pair_device_owned": (C.c_int, [C.c_void_p]),
 }
@@ -263,11 +265,17 @@ class Pair:
             raise RuntimeError(last_error())
         return out
 
-    def device_claim(self):
+    def device_claim(self, mirrored=True):
         """Hand this end to the caller's kernels (include/b200_device.cuh): returns the 64-byte b200_dev_pair
-        handle.  Host calls on this end are refused until device_release()."""
+        handle.  Host calls on this end are refused until device_release().  mirrored=False claims it with
+        B200_CLAIM_UNMIRRORED: nothing writes its host-visible mirror until the release, so its host readiness and
+        status queries stay as the claim left them."""
         buf = C.create_string_buffer(DEV_PAIR_BYTES)
-        if self.L.b200_pair_device_claim(self.h, buf) != 0:
+        if mirrored:
+            rc = self.L.b200_pair_device_claim(self.h, buf)
+        else:
+            rc = self.L.b200_pair_device_claim_ex(self.h, CLAIM_UNMIRRORED, buf)
+        if rc != 0:
             raise RuntimeError("b200_pair_device_claim failed: " + last_error())
         return buf.raw
 

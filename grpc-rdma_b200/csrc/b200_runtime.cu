@@ -120,6 +120,9 @@ struct b200_pair {
   // so one of the two always sees the other.
   std::atomic<bool> device_owned{false};
   std::atomic<int> host_ops{0};
+  // claimed with B200_CLAIM_UNMIRRORED: the row's mirror (and, loopback wire, the peer row's peer_mirror) is null
+  // until the release, so nothing writes this end's PairMirror
+  std::atomic<bool> unmirrored{false};
 };
 
 static const char* const kDeviceOwnedRefusal =
@@ -967,8 +970,10 @@ extern "C" void b200_pair_disconnect(b200_pair* p) {
     b200_pair* q = p->peer_local;
     cudaMemcpyAsync(&r.d_pairs[q->slot].credit_head, &st, 16, cudaMemcpyHostToDevice, r.stream);
     cudaStreamSynchronize(r.stream);
-    q->mirror->credit_head = st.remote_head;
-    q->mirror->peer_exit = 1;
+    if (!q->unmirrored.load()) {  // (an unmirrored end's release publishes it from the credit block)
+      q->mirror->credit_head = st.remote_head;
+      q->mirror->peer_exit = 1;
+    }
   }
   if (p->remote && was_connected) {  // the same 16-byte status write, over NVLink into the peer's table
     cudaStreamSynchronize(r.stream);
@@ -1538,13 +1543,14 @@ static uint64_t svc_recv(Runtime& r, b200_pair* p, void* dst, uint64_t cap) {
 // ================================================================ device API
 
 // The host-visible mirror of p from the device state (readiness as rx_probe computes it).  dev_closed is left as it
-// is: only b200_warp_disconnect sets it, Init clears it with the rest of the mirror.
-static void republish_mirror(Runtime& r, b200_pair* p) {
+// is: b200_warp_disconnect sets it (the release of an unmirrored end does, from the row), Init clears it with the
+// rest of the mirror.  Returns the row's status (-1 when the device could not be read).
+static int republish_mirror(Runtime& r, b200_pair* p) {
   PairDev hd;
   PairSeq sq;
   if (!CU_OK(cudaMemcpy(&hd, &r.d_pairs[p->slot], sizeof(hd), cudaMemcpyDeviceToHost)) ||
       !CU_OK(cudaMemcpy(&sq, pair_seq(r.d_pairs, p->slot), sizeof(sq), cudaMemcpyDeviceToHost)))
-    return;
+    return -1;
   uint32_t hm = 0;
   uint64_t rd = 0;
   if (hd.remain > 0) {
@@ -1553,7 +1559,7 @@ static void republish_mirror(Runtime& r, b200_pair* p) {
   } else if (hd.ring) {
     const uint32_t st = (hd.max_sge & kSgeStamped) ? stamp_of(sq.rx) : 0;
     uint64_t hdr = 0, foot = 0;
-    if (!CU_OK(cudaMemcpy(&hdr, hd.ring + hd.head, 8, cudaMemcpyDeviceToHost))) return;
+    if (!CU_OK(cudaMemcpy(&hdr, hd.ring + hd.head, 8, cudaMemcpyDeviceToHost))) return -1;
     hm = hdr != 0;
     const uint64_t len = frame_present(hdr, hd.cap, st);
     if (len && CU_OK(cudaMemcpy(&foot, hd.ring + ((hd.head + 8 + round_up8(len)) & (hd.cap - 1)), 8,
@@ -1572,9 +1578,29 @@ static void republish_mirror(Runtime& r, b200_pair* p) {
   m->credit_head = hd.credit_head;
   m->partial_write = hd.partial_write;
   m->peer_exit = hd.credit_exit;
+  return (int)hd.status;
 }
 
-extern "C" int b200_pair_device_claim(b200_pair* p, b200_dev_pair* out) {
+// The mirror pointers of p's row and, on the loopback wire, of its peer's row (peer_mirror): null for an unmirrored
+// claim, p->mirror again at its release.  The peer's row is left alone once the peer has left the connection.
+// Caller holds r.mu.
+static bool set_mirror_pointers(Runtime& r, b200_pair* p, bool on) {
+  PairMirror* const m = on ? p->mirror : nullptr;
+  bool ok = CU_OK(cudaMemcpyAsync(&r.d_pairs[p->slot].mirror, &m, sizeof(m), cudaMemcpyHostToDevice, r.stream));
+  b200_pair* q = p->peer_local;
+  if (q && q->peer_local == p)
+    ok = ok && CU_OK(cudaMemcpyAsync(&r.d_pairs[q->slot].peer_mirror, &m, sizeof(m), cudaMemcpyHostToDevice, r.stream));
+  return CU_OK(cudaStreamSynchronize(r.stream)) && ok;
+}
+
+extern "C" int b200_pair_device_claim(b200_pair* p, b200_dev_pair* out) { return b200_pair_device_claim_ex(p, 0, out); }
+
+extern "C" int b200_pair_device_claim_ex(b200_pair* p, int flags, b200_dev_pair* out) {
+  if (flags & ~B200_CLAIM_UNMIRRORED) {
+    set_err("b200_pair_device_claim_ex: unknown flag bits");
+    return -1;
+  }
+  const bool unmirrored = (flags & B200_CLAIM_UNMIRRORED) != 0;
   if (!p || !out || !ensure_init()) {
     set_err("b200_pair_device_claim: no pair / no output / no CUDA device");
     return -1;
@@ -1598,6 +1624,28 @@ extern "C" int b200_pair_device_claim(b200_pair* p, b200_dev_pair* out) {
   drain_retire(p);  // (an eager Recv that finished between the first drain and the claim)
   {
     std::lock_guard<std::mutex> lk(r.mu);
+    if (unmirrored) {
+      // A host op of the loopback peer may have loaded this end's mirror pointer before it goes null and publish
+      // through it afterwards: refused while one is in flight.  An op counted after this check starts after the
+      // pointers are null (single calls wait for r.mu, held here).  On the CUDA-IPC wire the host scans publish an
+      // end's mirror: none runs while scan_mu is held.
+      b200_pair* q = p->peer_local;
+      if (q && q->host_ops.load() != 0) {
+        p->device_owned = false;
+        set_err("b200_pair_device_claim_ex: host operations on the peer end are in flight");
+        return -1;
+      }
+      std::unique_lock<std::mutex> sl(r.scan_mu, std::defer_lock);
+      if (p->remote) sl.lock();
+      cudaSetDevice(r.dev);
+      if (!set_mirror_pointers(r, p, false)) {
+        set_mirror_pointers(r, p, true);
+        p->device_owned = false;
+        set_err("b200_pair_device_claim_ex: " + std::string(t_err));
+        return -1;
+      }
+      p->unmirrored = true;
+    }
     r.dev_slot[p->slot] = 1;
     if (r.svc_running.load()) memset((void*)&r.svc_erec[p->slot], 0, sizeof(EagerRec));  // no eager Recv any more
     ((volatile PairMirror*)p->mirror)->dev_closed = 0;  // (a CONNECTED end: clear since Init; set only by the device)
@@ -1619,6 +1667,27 @@ extern "C" int b200_pair_device_claim(b200_pair* p, b200_dev_pair* out) {
       c->flags = B200_BATCH_ONE_CALL;
     });
     svc_wait(r, q, t, nullptr, nullptr);
+    if (unmirrored && p->remote) {
+      // the device poller publishes the mirrors of CUDA-IPC ends: a scan that loaded the pointer before it went null
+      // may publish once more.  Two completed scans later none can; the mirror is then rebuilt from the device.  The
+      // wait does not hold r.mu: the other pairs' host calls go on meanwhile.
+      uint32_t s0 = 0, s = 0;
+      cudaMemcpyAsync(&s0, &r.d_svc_ps->scans, 4, cudaMemcpyDeviceToHost, r.stream);
+      cudaStreamSynchronize(r.stream);
+      const auto until = std::chrono::steady_clock::now() + std::chrono::seconds(5);
+      do {
+        std::this_thread::sleep_for(std::chrono::microseconds(20));
+        cudaMemcpyAsync(&s, &r.d_svc_ps->scans, 4, cudaMemcpyDeviceToHost, r.stream);
+        cudaStreamSynchronize(r.stream);
+      } while (s - s0 < 2 && std::chrono::steady_clock::now() < until);
+      std::lock_guard<std::mutex> lk(r.mu);
+      if (s - s0 < 2) {
+        device_release_locked(r, p);
+        set_err("b200_pair_device_claim_ex: the device poller did not complete a scan");
+        return -1;
+      }
+      republish_mirror(r, p);
+    }
   }
   return 0;
 }
@@ -1628,13 +1697,22 @@ extern "C" int b200_pair_device_claim(b200_pair* p, b200_dev_pair* out) {
 static void device_release_locked(Runtime& r, b200_pair* p) {
   if (!p->device_owned.load()) return;
   cudaSetDevice(r.dev);
+  const bool unmirrored = p->unmirrored.load();
+  if (unmirrored) {
+    // publication resumes before the mirror is rebuilt from the device, so no update falls between the two
+    set_mirror_pointers(r, p, true);
+    p->unmirrored = false;
+  }
   if (r.svc_running.load()) {
     const PairSvc fresh{p->svc_delivered, ~0ull};
     memset((void*)&r.svc_erec[p->slot], 0, sizeof(EagerRec));
     cudaMemcpyAsync(&r.d_svc_psvc[p->slot], &fresh, sizeof(fresh), cudaMemcpyHostToDevice, r.stream);
     cudaStreamSynchronize(r.stream);
   }
-  republish_mirror(r, p);
+  const int row_status = republish_mirror(r, p);
+  // an unmirrored end's b200_warp_disconnect could not set the mirror's flag: the row's status tells
+  if (unmirrored && p->status == B200_CONNECTED && row_status == B200_DISCONNECTED)
+    ((volatile PairMirror*)p->mirror)->dev_closed = 1;
   r.svc_gen++;
   r.dev_slot[p->slot] = 0;
   p->device_owned = false;

@@ -488,9 +488,12 @@ __device__ inline uint64_t warp_send_call(PairDev* table, int slot, const SliceD
     if (stamped) VL(S->tx) = tx + nframes;
     VL(P->remote_tail) = (rt + esum) & mask;
     VL(P->partial_write) = written < total;  // pair.cc:712
-    mirror_lock(P, true);
-    publish_mirror_tx(VL(P->mirror), P);
-    mirror_unlock(P, true);
+    PairMirror* pm = VL(P->mirror);  // null: an end claimed with B200_CLAIM_UNMIRRORED, nothing to publish
+    if (pm) {
+      mirror_lock(P, true);
+      publish_mirror_tx(pm, P);
+      mirror_unlock(P, true);
+    }
     const int peer_slot = VL(P->peer_slot);  // loopback wire: the peer's readiness hint
     if (peer_slot >= 0 && written) {
       PairDev* Q = table + peer_slot;
@@ -536,10 +539,10 @@ __device__ inline uint64_t warp_recv_call(PairDev* table, int slot, uint8_t* dst
   if (lane == 0) {
     if (credit) {  // updateStatus, pair.cc:624-641: the 16-byte status_report
       const int peer_slot = VL(Q->peer_slot);
-      PairDev* Pp = peer_slot >= 0 ? table + peer_slot : nullptr;
+      PairMirror* pm = VL(Q->peer_mirror);  // (loopback wire; null when the peer end is claimed unmirrored)
+      PairDev* Pp = peer_slot >= 0 && pm ? table + peer_slot : nullptr;
       if (Pp) mirror_lock(Pp, true);
       asm volatile("st.global.v2.u64 [%0], {%1,%2};" ::"l"(VL(Q->peer_credit)), "l"(c.mh), "l"(0ull) : "memory");
-      PairMirror* pm = VL(Q->peer_mirror);
       if (pm) ((volatile PairMirror*)pm)->credit_head = c.mh;
       if (Pp) mirror_unlock(Pp, true);
     }
@@ -548,13 +551,16 @@ __device__ inline uint64_t warp_recv_call(PairDev* table, int slot, uint8_t* dst
     VL(Q->remain) = c.remain;
     VL(Q->acc) = c.acc;
     if (stamped) VL(S->rx) = c.rx;
-    uint32_t hm;
-    uint64_t rd;
-    mirror_lock(Q, true);
-    if (sys) rx_probe<true>(ring, cap, c.head, c.remain, stamped ? stamp_of(c.rx) : 0, hm, rd);
-    else rx_probe<false>(ring, cap, c.head, c.remain, stamped ? stamp_of(c.rx) : 0, hm, rd);
-    publish_mirror_rx(VL(Q->mirror), Q, hm, rd);
-    mirror_unlock(Q, true);
+    PairMirror* m = VL(Q->mirror);  // null: claimed unmirrored, nothing to publish
+    if (m) {
+      uint32_t hm;
+      uint64_t rd;
+      mirror_lock(Q, true);
+      if (sys) rx_probe<true>(ring, cap, c.head, c.remain, stamped ? stamp_of(c.rx) : 0, hm, rd);
+      else rx_probe<false>(ring, cap, c.head, c.remain, stamped ? stamp_of(c.rx) : 0, hm, rd);
+      publish_mirror_rx(m, Q, hm, rd);
+      mirror_unlock(Q, true);
+    }
   }
   __syncwarp();
   return n;
@@ -630,7 +636,8 @@ __device__ __forceinline__ uint64_t pair_writable(PairDev* table, int slot) {
 // end wrote is visible before the peer can see the close; (2) unless the peer has left already, the 16-byte
 // status_report {moving_head, peer_exit = 1} into the peer's credit block -- on the loopback wire with the peer's
 // mirror, under the peer's mirror lock; (3) the row's status = DISCONNECTED, so every later call on the end refuses;
-// (4) the end's mirror flag that tells the host the rest of the Disconnect is due at the release.  Returns 1.
+// (4) the end's mirror flag that tells the host the rest of the Disconnect is due at the release (an end claimed
+// unmirrored has no mirror: its release finds the DISCONNECTED row instead).  Returns 1.
 __device__ inline int warp_disconnect(PairDev* table, int slot, uint32_t lane) {
   PairDev* P = table + slot;
   uint32_t st = 0;
@@ -643,10 +650,10 @@ __device__ inline int warp_disconnect(PairDev* table, int slot, uint32_t lane) {
     if (ld_acquire_u32(&P->credit_exit) != 1) {
       const uint64_t mh = VL(P->moving_head);
       const int peer_slot = VL(P->peer_slot);
-      PairDev* Q = peer_slot >= 0 ? table + peer_slot : nullptr;
+      PairMirror* pm = VL(P->peer_mirror);
+      PairDev* Q = peer_slot >= 0 && pm ? table + peer_slot : nullptr;
       if (Q) mirror_lock(Q, true);
       asm volatile("st.global.v2.u64 [%0], {%1,%2};" ::"l"(VL(P->peer_credit)), "l"(mh), "l"(1ull) : "memory");
-      PairMirror* pm = VL(P->peer_mirror);
       if (pm) {
         volatile PairMirror* vm = pm;
         vm->credit_head = mh;
@@ -655,9 +662,11 @@ __device__ inline int warp_disconnect(PairDev* table, int slot, uint32_t lane) {
       if (Q) mirror_unlock(Q, true);
     }
     VL(P->status) = kStDisconnected;
-    PairMirror* m = VL(P->mirror);
-    __threadfence_system();
-    if (m) ((volatile PairMirror*)m)->dev_closed = 1;
+    PairMirror* m = VL(P->mirror);  // null (claimed unmirrored): the release reads the row's status instead
+    if (m) {
+      __threadfence_system();
+      ((volatile PairMirror*)m)->dev_closed = 1;
+    }
   }
   __syncwarp();
   return 1;

@@ -24,7 +24,9 @@
  *     must have finished before the release.
  * At the end of each call the warp publishes the pair's host-visible mirror (and, on the loopback wire, the
  * peer's readiness and credit fields) under the per-pair mirror lock, so host readiness queries, the Poller and a
- * host-driven peer see the device-driven traffic.
+ * host-driven peer see the device-driven traffic.  An end claimed with B200_CLAIM_UNMIRRORED (b200_pair_device_claim_ex)
+ * has no mirror until its release: its calls skip its publication and its lock, and a peer's calls skip it too; the
+ * peer's own mirror is published as above.  The results are the same, bit for bit.
  *
  * The code behind these calls (include'd below) is the one the library's service owner warps run.
  */

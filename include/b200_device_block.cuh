@@ -30,7 +30,9 @@
  * other (a sender CTA and a receiver CTA of one connection) must make sure they are co-resident, and bounds its own
  * retry loops.  When b200_block_recv returns, the delivered bytes are visible to every thread of the calling CTA; a
  * consumer in another CTA or kernel needs the usual GPU-scope fence.  Every call publishes the pair's host-visible
- * mirror (and, on the loopback wire, the peer's readiness or credit) under the per-pair mirror lock.
+ * mirror (and, on the loopback wire, the peer's readiness or credit) under the per-pair mirror lock.  A mirror that an
+ * unmirrored claim (B200_CLAIM_UNMIRRORED) took away is skipped; with neither this end's nor its loopback peer's mirror
+ * left, the call takes no lock at all.  The results are the same, bit for bit.
  *
  * Refusals return 0 (and *calls = 0) to every thread and change nothing: a block shape other than
  * B200_BLOCK_THREADS x 1 x 1, any flag bit other than B200_BATCH_UNTIL_BLOCKED, a pair that is not connected, a Send
@@ -67,6 +69,16 @@ typedef struct b200_block {
 // its start, as k_send does, so that their addresses are constants: a base kept in a register costs k_send's body six
 // registers.
 extern __shared__ __align__(128) uint8_t b200_block_stages[];
+
+// The op's publication flag: kFlagConcurrent makes the bodies publish the mirrors under the per-pair locks.  When
+// neither this end nor its loopback peer has a mirror -- both ends of a loopback connection claimed with
+// B200_CLAIM_UNMIRRORED, or a CUDA-IPC end claimed so (such an end has no peer row here) -- the bodies have nothing to
+// publish, and the flag, whose only effect is the locks, is left out.  Every mirrored end keeps it, on either wire.
+__device__ __forceinline__ uint32_t b200_publish_flag(const b200::PairDev* P) {
+  return *(volatile b200::PairMirror* const*)&P->mirror || *(volatile b200::PairMirror* const*)&P->peer_mirror
+             ? b200::kFlagConcurrent
+             : 0u;
+}
 
 __device__ __forceinline__ bool b200_block_shape_ok() {
   return blockDim.x == B200_BLOCK_THREADS && blockDim.y == 1 && blockDim.z == 1;
@@ -114,7 +126,7 @@ __device__ inline uint64_t b200_block_send(b200_block* st, const b200_dev_pair* 
              b200::ld_acquire_u32(&P->credit_exit) != 1;
     b200::SendOpDev& op = st->sop;
     op.slot = h->slot;
-    op.flags = (uint32_t)flags | b200::kFlagConcurrent;  // a device-owned end publishes under the per-pair lock
+    op.flags = (uint32_t)flags | b200_publish_flag(P);  // a device-owned end publishes under the per-pair lock
     op.slices = reinterpret_cast<const b200::SliceDev*>(slices);
     op.nslices = n;
     op.byte_idx = byte_idx;
@@ -137,7 +149,7 @@ __device__ inline uint64_t b200_block_recv(b200_block* st, const b200_dev_pair* 
     st->go = *(volatile const uint32_t*)&table[h->slot].status == b200::kStConnected && cap != 0;  // pair.cc:266-268
     b200::RecvOpDev& op = st->rop;
     op.slot = h->slot;
-    op.flags = (uint32_t)flags | b200::kFlagConcurrent;
+    op.flags = (uint32_t)flags | b200_publish_flag(table + h->slot);
     op.dst = static_cast<uint8_t*>(dst);
     op.cap = cap;
   }
@@ -225,7 +237,7 @@ __device__ inline uint64_t b200_cluster_send(b200_block* st, const b200_dev_pair
     st->table = table;
     b200::SendOpDev& op = st->sop;
     op.slot = h->slot;
-    op.flags = (uint32_t)flags | b200::kFlagConcurrent;
+    op.flags = (uint32_t)flags | b200_publish_flag(P);
     op.slices = reinterpret_cast<const b200::SliceDev*>(slices);
     op.nslices = n;
     op.byte_idx = byte_idx;
@@ -250,7 +262,7 @@ __device__ inline uint64_t b200_cluster_recv(b200_block* st, const b200_dev_pair
     st->table = table;
     b200::RecvOpDev& op = st->rop;
     op.slot = h->slot;
-    op.flags = (uint32_t)flags | b200::kFlagConcurrent;
+    op.flags = (uint32_t)flags | b200_publish_flag(table + h->slot);
     op.dst = static_cast<uint8_t*>(dst);
     op.cap = cap;
   }

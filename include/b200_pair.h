@@ -202,6 +202,27 @@ typedef struct b200_dev_pair {
   uint64_t _reserved[4];
 } b200_dev_pair;   /* POD, 64 bytes: pass it by pointer (device or pinned memory) or by value */
 int b200_pair_device_claim(b200_pair* p, b200_dev_pair* out);
+/*
+ * b200_pair_device_claim_ex: b200_pair_device_claim with flags; b200_pair_device_claim(p, out) is
+ * b200_pair_device_claim_ex(p, 0, out).  Unknown flag bits: -1 and b200_last_error.
+ * B200_CLAIM_UNMIRRORED: while the end is claimed, nothing writes its host-visible mirror -- not the device calls of
+ * either end, the service, the Poller nor the host calls of the peer.  For a connection whose bytes never leave the
+ * GPU this takes the per-call publication (PCIe stores, system-scope fences, the per-pair mirror lock) off the device
+ * calls.  Every data result is the mirrored claim's, bit for bit, in every framing mode.  The peer end keeps its own
+ * mirror as before: a host-driven peer still sees its readiness after our Send and its credit after our Recv.
+ *   - Frozen queries: b200_pair_status, b200_pair_has_message / has_pending_writes / readable / writable on this end
+ *     answer from the mirror as the claim left it, until the release (a device Disconnect of the end included).
+ *     get_state and copy_ring read the device and keep working; the kernel has the device queries of
+ *     b200_device.cuh.
+ *   - Refused (-1) besides the plain claim's refusals: while the loopback peer has a host op in flight.  A peer end
+ *     that a kernel drives must not be inside a call at the claim.
+ *   - On the CUDA-IPC wire with the service running, the claim waits for the device poller's scans in progress to
+ *     pass, then rebuilds the frozen mirror from the device state.
+ *   - b200_pair_device_release publishes again: the mirror is rebuilt from the device state, and a Disconnect the
+ *     device made (b200_warp_disconnect) is finished as on a mirrored end.
+ */
+#define B200_CLAIM_UNMIRRORED 0x1
+int b200_pair_device_claim_ex(b200_pair* p, int flags, b200_dev_pair* out);
 int b200_pair_device_release(b200_pair* p);
 /* 1 while the pair is device-owned */
 int b200_pair_device_owned(const b200_pair* p);
