@@ -1362,8 +1362,8 @@ extern "C" uint64_t b200_service_eager_hits(void) { return R().svc_eager_hits.lo
 extern "C" int b200_debug_service_trace(unsigned long long* out16) { return svc_trace_read(out16); }
 
 // Where a Send stages its unregistered slices: [base, base + cap), filled from off.  grow: the calling thread's tx
-// buffer, grown at the first unregistered slice to everything one call can read (the ring plus a 16-byte step per
-// slice of the larger window; kCoalesceSlices >= kMaxSgeLimit).
+// buffer, grown at the first unregistered slice to the ring plus a 16-byte step per slice of the larger window
+// (kCoalesceSlices >= kMaxSgeLimit), more than a one-call op stages.
 struct SendStage {
   uint8_t* base;
   uint64_t cap, off;
@@ -1375,53 +1375,79 @@ constexpr uint64_t kSendSlack = 16ull * (kCoalesceSlices + 4);
 // kSvcSliceArea - 1) are looked at (*nreal), the rest only counts towards total_slice_size (pair.cc:661-664) and is
 // folded into one trailing pseudo-slice that is never dereferenced.  Unregistered host memory is copied to st like the
 // reference copies slices into its registered send buffer (pair.cc:690-694), in 16-byte steps, with (ptr + skip)
-// pointing at the staged bytes.  A one-call op stages at most C/2 bytes of a slice (coalesced: ONE frame of at most
-// CWS(C/2) bytes gathers all of them, so C/2 in all), and stages what fits of a slice that does not fit; an
-// until-blocked op ends its looked-at prefix at that slice.  Returns the number of entries, -1 when the staging
-// cannot be allocated.
+// pointing at the staged bytes.
+//   One call: the kernel never accepts more than C/2 bytes (one frame of at most CWS(C/2), or frames that share a
+//   C/2 staging size) and reads them from the front of the slices, so only the first C/2 bytes from byte_idx on are
+//   staged: at most C/2 plus a 16-byte step per looked-at slice.  st must hold all of it (-1 otherwise).
+//   Until blocked: the looked-at slices are staged whole while they fit.  The slice that does not fit is staged as far
+//   as st reaches and its entry shortened; the rest of it is folded into the pseudo-slice with what follows, so
+//   total_slice_size is unchanged and the op stops at the end of the staged prefix as if the ring had filled there.
+//   A slice that finds st full ends the prefix before it.
+// out == nullptr measures: nothing is copied or written, st.off ends at the bytes the op stages (stage_need).
+// Returns the number of entries, -1 when the staging cannot be allocated or does not hold a one-call op.
 static long stage_send(const b200_pair* p, SliceDev* out, const b200_slice* slices, size_t n, size_t byte_idx,
                        bool one_call, SendStage& st, size_t* nreal) {
   size_t look = one_call ? (p->coalesce ? kCoalesceSlices : (size_t)p->max_sge) : kSvcSliceArea - 1;
   if (look > n) look = n;
-  uint64_t budget = p->cap / 2;
+  uint64_t budget = p->cap / 2;  // one call: bytes the kernel may still read, in slice order
+  uint64_t cut = 0;              // until blocked: bytes of the last looked-at slice beyond the staged prefix
   for (size_t i = 0; i < look; i++) {
     const uint8_t* ptr = (const uint8_t*)slices[i].ptr;
     const uint64_t len = slices[i].len;
-    out[i].ptr = ptr;
-    out[i].len = len;
-    if (!len || mem_kind(ptr) != 0) continue;
     const uint64_t skip = i == 0 ? byte_idx : 0;
-    uint64_t take = len - skip;
+    uint64_t take = len > skip ? len - skip : 0;
     if (one_call) {
-      if (take > p->cap / 2) take = p->cap / 2;  // a call never accepts more than the staging size
-      if (p->coalesce) {
-        if (take > budget) take = budget;
-        budget -= take;
-      }
+      if (take > budget) take = budget;
+      budget -= take;
     }
+    if (out) out[i] = SliceDev{ptr, len};
+    if (!len || mem_kind(ptr) != 0) continue;
     if (st.grow) {
       TlsBounce& tb = tls_bounce();
       if (!ensure_bounce(&tb.tx, &tb.tx_cap, p->cap + kSendSlack)) return -1;
       st = SendStage{tb.tx, tb.tx_cap, 0, false};
     }
-    if (st.off + take > st.cap) {
-      if (!one_call) {
-        look = i;  // staged prefix only; the rest only counts towards total_slice_size
+    const uint64_t room = st.cap > st.off ? st.cap - st.off : 0;
+    bool last = false;
+    if (take > room) {
+      if (one_call) {
+        set_err("stage_send: the staging buffer does not hold what one call reads");
+        return -1;
+      }
+      if (!room) {
+        look = i;
         break;
       }
-      take = st.cap - st.off;
+      cut = take - room;
+      take = room;
+      last = true;
     }
-    memcpy(st.base + st.off, ptr + skip, take);
-    out[i].ptr = st.base + st.off - skip;
+    if (out) {
+      memcpy(st.base + st.off, ptr + skip, take);
+      out[i].ptr = st.base + st.off - skip;
+      if (last) out[i].len = skip + take;
+    }
     st.off += (take + 15) & ~15ull;
+    if (last) {
+      look = i + 1;
+      break;
+    }
   }
   *nreal = look;
-  uint64_t rest = 0;
+  uint64_t rest = cut;
   for (size_t i = look; i < n; i++) rest += slices[i].len;
-  if (!rest) return (long)look;
+  if (!rest || !out) return (long)look;
   out[look].ptr = nullptr;
   out[look].len = rest;
   return (long)look + 1;
+}
+
+// The bytes stage_send stages for this op: what its SendStage must hold to stage it whole
+static uint64_t stage_need(const b200_pair* p, const b200_slice* slices, size_t n, size_t byte_idx, bool one_call) {
+  SendStage st{nullptr, ~0ull, 0, false};
+  size_t nreal = 0;
+  stage_send(p, nullptr, slices, n, byte_idx, one_call, st, &nreal);
+  return st.off;
 }
 
 // A Send command that carries the pair's owed Retire (the owner warp runs it right after the Send), claimed inside
@@ -2227,10 +2253,11 @@ extern "C" int b200_pairs_recv(const b200_recv_op* ops, size_t nops, int flags, 
 // ------------------------------------------------------------------ device staging of service Recvs
 
 namespace {
-// device staging blocks of the service's Recvs (power-of-two classes) and finished posted-op handles, recycled
+// device staging blocks of the service's Recvs and pinned staging blocks of posted Sends (power-of-two classes: 2^31
+// bytes at most for a Recv, any size a one-call Send stages) and finished posted-op handles, recycled
 struct AsyncPool {
   std::mutex mu;
-  std::vector<uint8_t*> free_stage[32], free_hstage[32];
+  std::vector<uint8_t*> free_stage[32], free_hstage[64];
   std::vector<b200_async*> free_ops;
   cudaStream_t copy[4] = {nullptr, nullptr, nullptr, nullptr};
   std::atomic<uint32_t> rr{0};
@@ -2276,10 +2303,11 @@ cudaStream_t copy_stream() {
 // Recv) into pinned HOST memory (kind 1) of at least that size goes through a device staging block and ONE contiguous
 // D2H copy by the copy engine instead of SM stores over PCIe.  (SM-issued PCIe reads and writes share one ceiling,
 // tools/zc_overlap.py; on the endpoint streaming workload the staged form measured the same as the in-place form.)
-// nullptr: the Recv writes in place.  The block goes back with stage_put once its copy has finished.
+// nullptr: the Recv writes in place, as does one whose cap is larger than the largest block class (2^31 bytes).  The
+// block goes back with stage_put once its copy has finished.
 uint8_t* recv_stage(int kind, uint64_t cap, int* cls) {
   static const uint64_t kStageMin = (uint64_t)env_long("B200_SUBMIT_STAGE_MIN", 1l << 40);
-  if (kind != 1 || cap < kStageMin) return nullptr;
+  if (kind != 1 || cap < kStageMin || cap > (1ull << 31)) return nullptr;
   cudaSetDevice(R().dev);
   return stage_get(cap, cls);
 }
@@ -2328,16 +2356,26 @@ extern "C" int b200_pairs_submit(const b200_send_op* sops, size_t ns, uint64_t* 
   static thread_local std::vector<Ticket> st, rt;
   st.assign(ns, Ticket{0, 0, false});
   rt.assign(nr, Ticket{0, 0, false});
-  // staging for unregistered slices: one pinned buffer for the whole pass
-  uint64_t need = 0;
-  for (size_t i = 0; i < ns; i++)
-    for (size_t j = 0; j < sops[i].nslices && j < kSvcSliceArea; j++)
-      if (sops[i].slices[j].len && mem_kind(sops[i].slices[j].ptr) == 0) need += (sops[i].slices[j].len + 15) & ~15ull;
-  TlsBounce& tb = tls_bounce();
-  const uint64_t kMaxBounce = 1ull << 30;
-  if (need && !ensure_bounce(&tb.tx, &tb.tx_cap, need < kMaxBounce ? need : kMaxBounce)) return -1;
-  SendStage stage{tb.tx, tb.tx_cap, 0, false};
+  // staging for unregistered slices: one pinned buffer for the whole pass, sized for what its Sends stage
+  // (stage_need), at most kMaxBounce unless one one-call op stages more (it is staged whole or not at all).  A Send
+  // that does not fit in what is left waits for the pass's posted ops -- the only readers of the buffer -- and
+  // starts it again from the front; an until-blocked op larger than the buffer stages a prefix.
   const uint32_t fl = (uint32_t)(flags & (B200_BATCH_UNTIL_BLOCKED));
+  static thread_local std::vector<uint64_t> sneed;
+  sneed.assign(ns, 0);
+  uint64_t need = 0, most = 0;
+  for (size_t i = 0; i < ns; i++) {
+    if (!sops[i].pair || !sops[i].nslices) continue;
+    sneed[i] = stage_need(sops[i].pair, sops[i].slices, sops[i].nslices, sops[i].byte_idx, !fl);
+    need += sneed[i];
+    if (sneed[i] > most) most = sneed[i];
+  }
+  const uint64_t kMaxBounce = 1ull << 30;
+  uint64_t size = need < kMaxBounce ? need : kMaxBounce;
+  if (!fl && size < most) size = most;
+  TlsBounce& tb = tls_bounce();
+  if (size && !ensure_bounce(&tb.tx, &tb.tx_cap, size)) return -1;
+  SendStage stage{tb.tx, tb.tx_cap, 0, false};
   int rc = 0;
   static thread_local std::vector<uint8_t*> rstage;  // device staging of a Recv (recv_stage), by op
   static thread_local std::vector<int> rcls;
@@ -2377,6 +2415,10 @@ extern "C" int b200_pairs_submit(const b200_send_op* sops, size_t ns, uint64_t* 
       drain_retire(p->peer_local);
     }
     if (send_is_a_no_op(p)) continue;
+    if (stage.off && sneed[i] > stage.cap - stage.off) {
+      harvest();
+      stage.off = 0;
+    }
     const int q = owner_of(r, p);
     auto fill = [&](SvcCmd* c, SliceDev* area) {
       fill_send_cmd(p, c, area, sops[i].slices, sops[i].nslices, sops[i].byte_idx, fl, stage);
@@ -2494,13 +2536,14 @@ extern "C" b200_async* b200_pair_post_send(b200_pair* p, const b200_slice* slice
   if (send_is_a_no_op(p)) return o;
   const int q = owner_of(r, p);
   uint64_t t = 0;
-  {  // unregistered slices are staged in pinned memory that belongs to the op
-    uint64_t need = 0;
-    for (size_t i = 0; i < n && i < kSvcSliceArea; i++)
-      if (slices[i].len && mem_kind(slices[i].ptr) == 0) need += (slices[i].len + 15) & ~15ull;
+  const uint32_t fl = (uint32_t)(flags & B200_BATCH_UNTIL_BLOCKED);
+  {  // unregistered slices are staged in pinned memory that belongs to the op: a block of the power-of-two class of
+     // what it stages (stage_need).  A one-call op's block holds all of it; an until-blocked op's is at most 2^28
+     // bytes, and when it needs more it stages a prefix.
+    const uint64_t need = stage_need(p, slices, n, byte_idx, !fl);
     if (need) {
       int c = 12;
-      while ((1ull << c) < need && c < 28) c++;
+      while ((1ull << c) < need && (c < 28 || !fl)) c++;
       AsyncPool& a = AP();
       {
         std::lock_guard<std::mutex> lk(a.mu);
@@ -2523,7 +2566,7 @@ extern "C" b200_async* b200_pair_post_send(b200_pair* p, const b200_slice* slice
   }
   SendStage st{o->hstage, o->hstage ? 1ull << o->hstage_cls : 0, 0, false};
   auto fill = [&](SvcCmd* c, SliceDev* area) {
-    fill_send_cmd(p, c, area, slices, n, byte_idx, (uint32_t)(flags & B200_BATCH_UNTIL_BLOCKED), st);
+    fill_send_cmd(p, c, area, slices, n, byte_idx, fl, st);
   };
   if (!svc_try_post(r, q, fill, &t)) {
     async_put(o);
