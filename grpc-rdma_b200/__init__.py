@@ -25,6 +25,7 @@ ENDPOINT_HEADER = os.path.join(ROOT, "include", "b200_endpoint.h")
 
 ADDRESS_BYTES = 48
 DEV_PAIR_BYTES = 64  # sizeof(b200_dev_pair)
+DEV_READY_SET_BYTES = 64  # sizeof(b200_dev_ready_set)
 CLAIM_UNMIRRORED = 0x1  # B200_CLAIM_UNMIRRORED (b200_pair_device_claim_ex)
 ONE_CALL, UNTIL_BLOCKED, ASYNC, ZEROCOPY = 0, 1, 2, 4
 EV_READABLE, EV_WRITABLE = 0x1, 0x4
@@ -136,6 +137,10 @@ _SIGS = {
     "b200_pair_device_claim_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "b200_pair_device_release": (C.c_int, [C.c_void_p]),
     "b200_pair_device_owned": (C.c_int, [C.c_void_p]),
+    "b200_ready_set_create": (C.c_void_p, [C.c_uint32]),
+    "b200_ready_set_device": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "b200_ready_set_destroy": (C.c_int, [C.c_void_p]),
+    "b200_ready_set_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32]),
 }
 
 _lib = None
@@ -292,6 +297,36 @@ class Pair:
 
     def putback(self):
         self.L.b200_pool_putback(self.h)
+
+
+class ReadySet:
+    """A device ready set (b200_ready_set_*): the queue a consumer kernel takes ready members' keys from
+    (include/b200_device.cuh: b200_warp_ready_take / b200_warp_ready_rearm).  Members are claimed Pairs on the loopback
+    wire; membership ends with the claim."""
+
+    def __init__(self, capacity):
+        self.L = lib()
+        self.h = self.L.b200_ready_set_create(capacity)
+        if not self.h:
+            raise RuntimeError("b200_ready_set_create failed: " + last_error())
+
+    def device(self):
+        """the 64-byte b200_dev_ready_set handle for kernels"""
+        buf = C.create_string_buffer(DEV_READY_SET_BYTES)
+        if self.L.b200_ready_set_device(self.h, buf) != 0:
+            raise RuntimeError(last_error())
+        return buf.raw
+
+    def add(self, pair, key):
+        """make the claimed `pair` a member with `key`; raises with b200_last_error's reason when refused"""
+        if self.L.b200_ready_set_add(self.h, pair.h, key) != 0:
+            raise RuntimeError("b200_ready_set_add failed: " + last_error())
+
+    def destroy(self):
+        """no kernel may use the set; raises while it has members"""
+        if self.L.b200_ready_set_destroy(self.h) != 0:
+            raise RuntimeError("b200_ready_set_destroy failed: " + last_error())
+        self.h = None
 
 
 def connected_pair(ident_a="a", ident_b="b"):

@@ -870,6 +870,7 @@ __device__ __forceinline__ void send_body(PairDev* __restrict__ pairs, const Sen
         mirror_unlock(Q, conc);
       }
     }
+    if (PS.written_total) notify_peer(pairs, peer_slot);  // (the footers are behind the last segment's barrier)
   }
 }
 
@@ -1297,6 +1298,7 @@ __device__ __forceinline__ void recv_body(PairDev* __restrict__ pairs, const Rec
       PairMirror* pm = VL(P->peer_mirror);
       if (pm) ((volatile PairMirror*)pm)->credit_head = SS.credit_val;
       if (conc) mirror_unlock(Q, true);
+      notify_peer(pairs, peer_slot);
       SS.credit_flag = 0;
     }
     pipe_sync<kCl>();

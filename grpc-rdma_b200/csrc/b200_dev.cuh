@@ -129,6 +129,50 @@ struct __align__(16) PairSeq {
 };
 B200_HD PairSeq* pair_seq(PairDev* table, int slot) { return reinterpret_cast<PairSeq*>(table + kMaxPairs) + slot; }
 
+// ---- device ready sets (b200_ready_set_*, DESIGN.md §13 "Ready sets").  A set is a queue of 32-bit member keys in
+// device memory with one consumer warp; the paths that change a member's readiness append its key (notify_peer).
+// Control words: the consumer's head and the producers' tail on separate lines, then the entries.
+struct __align__(128) ReadyQueue {
+  uint32_t head;  // next position the consumer takes (written by the consumer only)
+  uint32_t _h[31];
+  uint32_t tail;  // next position a producer claims (atomicAdd)
+  uint32_t _t[31];
+  uint32_t mask;  // entries - 1, set at creation
+  uint32_t _m[31];
+};
+static_assert(sizeof(ReadyQueue) == 384, "ReadyQueue: three 128-byte lines");
+// An entry is one 8-byte word: the key, and position + 1 in the top half (0: never written), so the consumer tells a
+// written entry from a slot whose producer has claimed it but not yet stored into it.
+B200_HD uint64_t* ready_entries(ReadyQueue* q) { return reinterpret_cast<uint64_t*>(q + 1); }
+B200_HD uint64_t ready_entry(uint32_t key, uint32_t pos) { return (uint64_t)(pos + 1u) << 32 | key; }
+B200_HD bool ready_entry_at(uint64_t e, uint32_t pos) { return (uint32_t)(e >> 32) == pos + 1u; }
+// Entries of a set of `capacity` members: a power of two >= 2 * capacity.  Each member has at most one entry queued,
+// and an entry of a released member stays until it is taken, so twice the members leaves room for that many stale
+// entries before b200_ready_set_add has to refuse.
+B200_HD uint32_t ready_queue_size(uint32_t capacity) {
+  uint32_t s = 1;
+  while (s < 2 * capacity) s <<= 1;
+  return s;
+}
+constexpr int kReadyAddOk = 0, kReadyAddFull = 1, kReadyAddOverflow = 2;
+// May one more member join a set whose queue holds positions [head, tail)?  Each present member can still append one
+// entry and the new one appends its initial entry, so the entries in the queue plus the members must stay below its
+// size.  (tail - head) counts stale entries of released members as well.
+B200_HD int ready_add_check(uint32_t head, uint32_t tail, uint32_t members, uint32_t capacity, uint32_t size) {
+  if (members >= capacity) return kReadyAddFull;
+  return (uint64_t)(tail - head) + members < size ? kReadyAddOk : kReadyAddOverflow;
+}
+// The note of a ready-set member, in the side array that follows the PairSeq array of the connection table.  `set`
+// is null for an end that belongs to no set: the one load every producer pays.
+struct __align__(16) ReadyNote {
+  ReadyQueue* set;
+  uint32_t key;
+  uint32_t armed;  // 1: the next readiness change appends the key; 0: an entry is queued or the consumer holds the end
+};
+B200_HD ReadyNote* ready_note(PairDev* table, int slot) {
+  return reinterpret_cast<ReadyNote*>(pair_seq(table, kMaxPairs)) + slot;
+}
+
 struct SliceDev {  // same layout as b200_slice
   const uint8_t* ptr;
   uint64_t len;
@@ -279,6 +323,11 @@ void launch_recv(PairDev* pairs, const RecvOpDev* ops, OpResult* results, int no
 int cluster_capacity(int kind, int cluster);
 void launch_poll_scan(PairDev* pairs, const int32_t* slots, uint32_t* events, uint32_t* ready_count,
                       int32_t* ready_slots, int n, void* stream);
+// ready sets: load the library's kernels (before a user's consumer kernel may be resident); one-thread kernels that
+// make pair `slot` a member of `q` with `key`, and that run notify_peer for pair `slot` (b200_pair_disconnect)
+void load_kernels();
+void launch_ready_add(PairDev* pairs, int slot, ReadyQueue* q, uint32_t key, void* stream);
+void launch_ready_notify(PairDev* pairs, int slot, void* stream);
 
 // owners / pool / poller on three streams; returns false when the resident grids cannot be co-resident
 bool launch_service(const SvcParams& sp, void* s_owner, void* s_big, void* s_poll);

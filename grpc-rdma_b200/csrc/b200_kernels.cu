@@ -436,6 +436,8 @@ __device__ __forceinline__ void svc_send_small(const SvcParams& sp, const ConnVi
       vm->has_message = 1;
     }
   }
+  __syncwarp();  // (every lane's footer before lane 0's notify)
+  if (lane == 0 && wsum) notify_peer(sp.pairs, P.peer_slot);
   __syncwarp();
 }
 
@@ -553,6 +555,7 @@ __device__ __forceinline__ void svc_send_small_coalesced(const SvcParams& sp, co
       vm->has_message = 1;
     }
   }
+  if (lane == 0 && p) notify_peer(sp.pairs, P.peer_slot);  // (lane 0 wrote the footer)
   __syncwarp();
 }
 
@@ -587,6 +590,7 @@ __device__ __forceinline__ bool svc_recv_small(const SvcParams& sp, const ConnVi
     }
     if (lane == 0 && Q.peer_mirror) ((volatile PairMirror*)Q.peer_mirror)->credit_head = mh_after;
     if (lane == 0 && cv.Q) cv.Q->credit_head = mh_after;  // the cached line of the sender
+    if (lane == 0) notify_peer(sp.pairs, Q.peer_slot);
   }
   const uint64_t delivered = cv.SP->delivered + n;
   if (lane == 0) {
@@ -1047,6 +1051,22 @@ k_probe_copy(uint8_t* __restrict__ dst, uint8_t* __restrict__ src, uint64_t byte
   }
 }
 
+// =========================================================================
+// ready sets: one-thread library kernels (b200_ready_set_add, b200_pair_disconnect)
+// =========================================================================
+// k_ready_add: the note first, the set pointer last (a producer that finds the pointer finds the key), then one
+// initial entry with armed = 0, so that a frame or a close that came before the add is not lost.
+__global__ void k_ready_add(PairDev* pairs, int slot, ReadyQueue* q, uint32_t key) {
+  ReadyNote* n = ready_note(pairs, slot);
+  VL(n->key) = key;
+  VL(n->armed) = 0u;
+  __threadfence();
+  VL(n->set) = q;
+  __threadfence();
+  ready_push(q, key);
+}
+__global__ void k_ready_notify(PairDev* pairs, int slot) { notify_peer(pairs, slot); }
+
 static void ensure_kernel_attrs() {
   static std::once_flag once;
   std::call_once(once, [] {
@@ -1075,7 +1095,20 @@ static void ensure_kernel_attrs() {
   cudaFuncGetAttributes(&fa, k_svc_poll);
   cudaFuncGetAttributes(&fa, k_cluster_send);
   cudaFuncGetAttributes(&fa, k_cluster_recv);
+  cudaFuncGetAttributes(&fa, k_ready_add);
+  cudaFuncGetAttributes(&fa, k_ready_notify);
   });
+}
+
+void load_kernels() { ensure_kernel_attrs(); }
+
+void launch_ready_add(PairDev* pairs, int slot, ReadyQueue* q, uint32_t key, void* stream) {
+  ensure_kernel_attrs();
+  k_ready_add<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(pairs, slot, q, key);
+}
+void launch_ready_notify(PairDev* pairs, int slot, void* stream) {
+  ensure_kernel_attrs();
+  k_ready_notify<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(pairs, slot);
 }
 
 int svc_trace_read(unsigned long long* out16) {

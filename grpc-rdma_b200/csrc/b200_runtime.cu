@@ -123,6 +123,13 @@ struct b200_pair {
   // claimed with B200_CLAIM_UNMIRRORED: the row's mirror (and, loopback wire, the peer row's peer_mirror) is null
   // until the release, so nothing writes this end's PairMirror
   std::atomic<bool> unmirrored{false};
+  b200_ready_set* ready_set = nullptr;  // the set this claimed end is a member of (under the runtime lock)
+};
+
+struct b200_ready_set {
+  ReadyQueue* q = nullptr;  // device memory: control lines, then `size` entries
+  uint32_t capacity = 0, size = 0;
+  uint32_t members = 0;  // under the runtime lock
 };
 
 static const char* const kDeviceOwnedRefusal =
@@ -202,7 +209,7 @@ struct Runtime {
   cudaEvent_t send_done[kLanes] = {}, recv_done[kLanes] = {};
   cudaEvent_t join_up[kLanes] = {}, join_down[kLanes] = {};
   cudaEvent_t fork_event = nullptr;
-  PairDev* d_pairs = nullptr;       // kMaxPairs rows, then the kMaxPairs PairSeq of pair_seq()
+  PairDev* d_pairs = nullptr;       // kMaxPairs rows, then the kMaxPairs PairSeq of pair_seq(), then the ReadyNotes
   PairMirror* h_mirrors = nullptr;  // pinned, mapped
   std::vector<b200_pair*> all_pairs;
   std::queue<b200_pair*> pool;
@@ -463,7 +470,7 @@ static int init_locked(int device) {
       if (!CU_OK(cudaEventCreateWithFlags(e, cudaEventDisableTiming))) return -1;
   }
   if (!CU_OK(cudaEventCreateWithFlags(&r.fork_event, cudaEventDisableTiming))) return -1;
-  const size_t table_bytes = (sizeof(PairDev) + sizeof(PairSeq)) * kMaxPairs;
+  const size_t table_bytes = (sizeof(PairDev) + sizeof(PairSeq) + sizeof(ReadyNote)) * kMaxPairs;
   if (!CU_OK(cudaMalloc(&r.d_pairs, table_bytes))) return -1;
   if (!CU_OK(cudaMemset(r.d_pairs, 0, table_bytes))) return -1;
   if (!CU_OK(cudaHostAlloc(&r.h_mirrors, sizeof(PairMirror) * kMaxPairs, cudaHostAllocMapped | cudaHostAllocPortable)))
@@ -960,6 +967,11 @@ extern "C" void b200_pair_disconnect(b200_pair* p) {
     if (!q->unmirrored.load()) {  // (an unmirrored end's release publishes it from the credit block)
       q->mirror->credit_head = st.remote_head;
       q->mirror->peer_exit = 1;
+    }
+    if (q->ready_set) {  // the peer's readiness changed: its ready set hears of it
+      launch_ready_notify(r.d_pairs, q->slot, r.stream);
+      r.launches++;
+      cudaStreamSynchronize(r.stream);
     }
   }
   if (p->remote && was_connected) {  // the same 16-byte status write, over NVLink into the peer's table
@@ -1702,6 +1714,12 @@ extern "C" int b200_pair_device_claim_ex(b200_pair* p, int flags, b200_dev_pair*
 static void device_release_locked(Runtime& r, b200_pair* p) {
   if (!p->device_owned.load()) return;
   cudaSetDevice(r.dev);
+  if (p->ready_set) {  // membership ends with the claim: no producer finds the note from here on
+    cudaMemsetAsync(ready_note(r.d_pairs, p->slot), 0, sizeof(ReadyNote), r.stream);
+    cudaStreamSynchronize(r.stream);
+    p->ready_set->members--;
+    p->ready_set = nullptr;
+  }
   const bool unmirrored = p->unmirrored.load();
   if (unmirrored) {
     // publication resumes before the mirror is rebuilt from the device, so no update falls between the two
@@ -1738,6 +1756,102 @@ extern "C" int b200_pair_device_release(b200_pair* p) {
 }
 
 extern "C" int b200_pair_device_owned(const b200_pair* p) { return p && p->device_owned.load() ? 1 : 0; }
+
+// ================================================================ ready sets
+
+extern "C" b200_ready_set* b200_ready_set_create(uint32_t capacity) {
+  if (capacity < 1 || capacity > (uint32_t)kMaxPairs) {
+    set_err("b200_ready_set_create: capacity must be 1.." + std::to_string(kMaxPairs));
+    return nullptr;
+  }
+  if (!ensure_init()) return nullptr;
+  Runtime& r = R();
+  std::lock_guard<std::mutex> lk(r.mu);
+  cudaSetDevice(r.dev);
+  load_kernels();  // (a consumer kernel may be resident by the time of the first add)
+  b200_ready_set* s = new b200_ready_set();
+  s->capacity = capacity;
+  s->size = ready_queue_size(capacity);
+  const size_t bytes = sizeof(ReadyQueue) + sizeof(uint64_t) * s->size;
+  const uint32_t mask = s->size - 1;
+  if (!CU_OK(cudaMalloc(&s->q, bytes)) || !CU_OK(cudaMemsetAsync(s->q, 0, bytes, r.stream)) ||
+      !CU_OK(cudaMemcpyAsync(&s->q->mask, &mask, 4, cudaMemcpyHostToDevice, r.stream)) ||
+      !CU_OK(cudaStreamSynchronize(r.stream))) {
+    if (s->q) rt_free(s->q, 0);
+    delete s;
+    return nullptr;
+  }
+  return s;
+}
+
+extern "C" int b200_ready_set_device(b200_ready_set* s, b200_dev_ready_set* out) {
+  if (!s || !out) {
+    set_err("b200_ready_set_device: no set / no output");
+    return -1;
+  }
+  memset(out, 0, sizeof(*out));
+  out->queue = s->q;
+  out->capacity = s->capacity;
+  out->size = s->size;
+  return 0;
+}
+
+extern "C" int b200_ready_set_destroy(b200_ready_set* s) {
+  if (!s) return -1;
+  Runtime& r = R();
+  std::lock_guard<std::mutex> lk(r.mu);
+  if (s->members) {
+    set_err("b200_ready_set_destroy: the set has " + std::to_string(s->members) + " members");
+    return -1;
+  }
+  rt_free(s->q, 0);
+  delete s;
+  return 0;
+}
+
+extern "C" int b200_ready_set_add(b200_ready_set* s, b200_pair* p, uint32_t key) {
+  if (!s || !p) {
+    set_err("b200_ready_set_add: no set / no pair");
+    return -1;
+  }
+  Runtime& r = R();
+  std::lock_guard<std::mutex> lk(r.mu);
+  if (!p->device_owned.load()) {
+    set_err("b200_ready_set_add: the pair is not device-owned (b200_pair_device_claim)");
+    return -1;
+  }
+  if (p->remote || !p->peer_local) {
+    set_err("b200_ready_set_add: the pair is not on the loopback wire (its peer's kernels cannot reach the set)");
+    return -1;
+  }
+  if (p->ready_set) {
+    set_err("b200_ready_set_add: the pair is already a member of a ready set");
+    return -1;
+  }
+  cudaSetDevice(r.dev);
+  uint32_t head = 0, tail = 0;
+  if (!CU_OK(cudaMemcpyAsync(&head, &s->q->head, 4, cudaMemcpyDeviceToHost, r.stream)) ||
+      !CU_OK(cudaMemcpyAsync(&tail, &s->q->tail, 4, cudaMemcpyDeviceToHost, r.stream)) ||
+      !CU_OK(cudaStreamSynchronize(r.stream)))
+    return -1;
+  const int chk = ready_add_check(head, tail, s->members, s->capacity, s->size);
+  if (chk == kReadyAddFull) {
+    set_err("b200_ready_set_add: the set is full (" + std::to_string(s->capacity) + " members)");
+    return -1;
+  }
+  if (chk == kReadyAddOverflow) {
+    set_err("b200_ready_set_add: the queue could overflow: " + std::to_string(tail - head) +
+            " entries queued (stale entries of released members included) and " + std::to_string(s->members) +
+            " members against " + std::to_string(s->size) + " entries; take from the set first");
+    return -1;
+  }
+  launch_ready_add(r.d_pairs, p->slot, s->q, key, r.stream);
+  r.launches++;
+  if (!CU_OK(cudaGetLastError()) || !CU_OK(cudaStreamSynchronize(r.stream))) return -1;
+  s->members++;
+  p->ready_set = s;
+  return 0;
+}
 
 // ================================================================ single call
 

@@ -264,6 +264,26 @@ __device__ __forceinline__ void publish_mirror_locked(PairDev* table, int slot) 
   mirror_unlock(X, true);
 }
 
+// Ready sets (DESIGN.md §13 "Ready sets"), by ONE thread of a path that has just made a change of pair `peer_slot`'s
+// readiness visible: a frame's footer in its ring, the credit in its credit block, or its peer_exit.  An end that
+// belongs to no set costs the load of its note's set pointer.  A member: fence (the change before the exchange: with
+// the consumer's store / fence / probe in b200_warp_ready_rearm, Dekker's pattern), then whoever takes `armed` from 1
+// to 0 appends the key, so a member has at most one entry queued.  The entry is stored with release semantics after
+// the change, and the consumer loads it with acquire semantics.
+__device__ __forceinline__ void ready_push(ReadyQueue* q, uint32_t key) {
+  const uint32_t pos = atomicAdd(&q->tail, 1u);
+  uint64_t* e = ready_entries(q) + (pos & VL(q->mask));
+  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(e), "l"(ready_entry(key, pos)) : "memory");
+}
+__device__ __forceinline__ void notify_peer(PairDev* table, int peer_slot) {
+  if (peer_slot < 0) return;
+  ReadyNote* n = ready_note(table, peer_slot);
+  ReadyQueue* q = VL(n->set);
+  if (q == nullptr) return;
+  __threadfence();
+  if (atomicExch(&n->armed, 0u) == 1u) ready_push(q, VL(n->key));
+}
+
 // ======================================================================= one call by one warp, any size
 
 __device__ __forceinline__ uint64_t warp_sum(uint64_t v) {
@@ -510,6 +530,8 @@ __device__ inline uint64_t warp_send_call(PairDev* table, int slot, const SliceD
       }
     }
   }
+  __syncwarp();  // (every lane's footer before lane 0's notify)
+  if (lane == 0 && written) notify_peer(table, VL(P->peer_slot));
   __syncwarp();
   return written;
 }
@@ -545,6 +567,7 @@ __device__ inline uint64_t warp_recv_call(PairDev* table, int slot, uint8_t* dst
       asm volatile("st.global.v2.u64 [%0], {%1,%2};" ::"l"(VL(Q->peer_credit)), "l"(c.mh), "l"(0ull) : "memory");
       if (pm) ((volatile PairMirror*)pm)->credit_head = c.mh;
       if (Pp) mirror_unlock(Pp, true);
+      notify_peer(table, peer_slot);
     }
     VL(Q->head) = c.head;
     VL(Q->moving_head) = c.mh;
@@ -660,6 +683,7 @@ __device__ inline int warp_disconnect(PairDev* table, int slot, uint32_t lane) {
         vm->peer_exit = 1;
       }
       if (Q) mirror_unlock(Q, true);
+      notify_peer(table, peer_slot);
     }
     VL(P->status) = kStDisconnected;
     PairMirror* m = VL(P->mirror);  // null (claimed unmirrored): the release reads the row's status instead
@@ -670,6 +694,66 @@ __device__ inline int warp_disconnect(PairDev* table, int slot, uint32_t lane) {
   }
   __syncwarp();
   return 1;
+}
+
+// ======================================================================= ready sets: the consumer (one warp per set)
+
+// A member is ready when poll_events reports READABLE, or when it has a pending write and credit for at least one
+// frame: the inverse of the host's "this Send cannot accept a byte" rule.  (The Poller's level-triggered WRITABLE on
+// partial_write alone would hand a blocked sender back to an edge-triggered consumer at once, again and again.)
+__device__ __forceinline__ uint32_t ready_events(PairDev* table, int slot) {
+  const uint32_t ev = poll_events<false>(table, slot);
+  uint32_t out = ev & kEvReadable;
+  if (ev & kEvWritable) {  // (CONNECTED, the peer has not left, partial_write)
+    PairDev* P = table + slot;
+    const uint64_t cap = VL(P->cap);
+    const uint64_t fr = free_size(cap, ld_acquire_u64(&P->credit_head), VL(P->remote_tail));
+    if (calc_writable(fr < cap / 2 ? fr : cap / 2) != 0) out |= kEvWritable;
+  }
+  return out;
+}
+
+// Up to `max` keys from the head of the queue into keys[]; stops at the first position whose entry has not been
+// stored yet.  Returns how many, every lane.
+__device__ inline uint32_t ready_take(ReadyQueue* q, uint32_t* keys, uint32_t max, uint32_t lane) {
+  const uint32_t head = VL(q->head), mask = VL(q->mask);
+  uint32_t n = 0;
+  while (n < max) {
+    const uint32_t i = n + lane;
+    bool ok = false;
+    uint64_t e = 0;
+    if (i < max) {
+      const uint32_t pos = head + i;
+      asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(e) : "l"(ready_entries(q) + (pos & mask)) : "memory");
+      ok = ready_entry_at(e, pos);
+    }
+    const unsigned bad = __ballot_sync(0xffffffffu, !ok);
+    const uint32_t run = bad ? __ffs(bad) - 1 : 32;
+    if (lane < run) keys[i] = (uint32_t)e;
+    n += run;
+    if (run < 32) break;
+  }
+  __syncwarp();
+  if (lane == 0 && n) VL(q->head) = head + n;
+  __syncwarp();
+  return n;
+}
+
+// The consumer is done with member `slot` of `q`: armed = 1, a fence, then the probe.  Ready and the exchange won:
+// the member's events (the consumer keeps it, nothing is queued).  Otherwise 0: a producer that saw armed == 1 has
+// queued the key, or nothing is pending and the next change will.  0 as well for an end that is not a member of `q`.
+__device__ inline uint32_t ready_rearm(ReadyQueue* q, PairDev* table, int slot, uint32_t lane) {
+  uint32_t ev = 0;
+  if (lane == 0) {
+    ReadyNote* n = ready_note(table, slot);
+    if (VL(n->set) == q) {
+      VL(n->armed) = 1u;
+      __threadfence();
+      ev = ready_events(table, slot);
+      if (ev && atomicExch(&n->armed, 0u) != 1u) ev = 0;
+    }
+  }
+  return __shfl_sync(0xffffffffu, ev, 0);
 }
 
 }  // namespace b200

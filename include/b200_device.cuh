@@ -121,4 +121,28 @@ __device__ inline int b200_warp_disconnect(const b200_dev_pair* h) {
   return b200::warp_disconnect(reinterpret_cast<b200::PairDev*>(h->table), h->slot, b200_lane_id());
 }
 
+/* ---- ready sets: the device's epoll (b200_pair.h, DESIGN.md §13 "Ready sets") -------------------------------------
+ *
+ * A server warp that holds many claimed ends takes the keys of the ends whose readiness changed instead of scanning
+ * them all.  ONE consumer warp per set; neither call waits.
+ *   b200_warp_ready_take(s, keys, max): pops up to max keys into keys[] (device or pinned memory) and returns how many.
+ *     They are hints: the consumer drives those ends with the calls above (Recv until it returns 0, Send, Disconnect).
+ *     A taken key's frame, credit or close is visible to those calls.
+ *   b200_warp_ready_rearm(s, h): the consumer has finished with member h for now.  It stores armed = 1, fences and
+ *     probes.  When the end is READY (b200_warp_poll reports READABLE, or a write is pending and there is credit for
+ *     one frame) and the call wins the end back from the producers, it returns the end's B200_EV_* bits: the consumer
+ *     keeps the end and serves it again.  Otherwise 0: a producer has queued the key already, or nothing is pending
+ *     and the next change will queue it.  Every change after a rearm is reported, by the rearm itself or by an entry
+ *     (no lost wakeup), and a member never has two entries queued.
+ * The first entry of a member is queued by b200_ready_set_add, with the member disarmed: take it, serve, rearm.  An
+ * entry of a released member can still be taken once; its key then names an end that is no longer a member.
+ */
+__device__ inline uint32_t b200_warp_ready_take(const b200_dev_ready_set* s, uint32_t* keys, uint32_t max) {
+  return b200::ready_take(static_cast<b200::ReadyQueue*>(s->queue), keys, max, b200_lane_id());
+}
+__device__ inline uint32_t b200_warp_ready_rearm(const b200_dev_ready_set* s, const b200_dev_pair* h) {
+  return b200::ready_rearm(static_cast<b200::ReadyQueue*>(s->queue), reinterpret_cast<b200::PairDev*>(h->table),
+                           h->slot, b200_lane_id());
+}
+
 #endif /* B200_DEVICE_CUH */

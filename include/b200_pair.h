@@ -227,8 +227,51 @@ int b200_pair_device_release(b200_pair* p);
 /* 1 while the pair is device-owned */
 int b200_pair_device_owned(const b200_pair* p);
 
+/*
+ * Ready sets: the device's epoll (DESIGN.md §13 "Ready sets").  A polling server kernel that holds many claimed ends
+ * takes the ones whose readiness changed from a device queue, b200_warp_ready_take (b200_device.cuh), instead of
+ * scanning them all with b200_warp_poll.  Edge-triggered and one-shot, like EPOLLONESHOT with re-arm:
+ *   - members are claimed ends (either claim form) on the loopback wire, each with a 32-bit key the caller chooses; an
+ *     end belongs to at most one set;
+ *   - the peer's Send landing a frame, the peer's Recv returning credit and the peer's Disconnect (host or device)
+ *     append the member's key when the member is armed, and disarm it: a member has at most one entry queued;
+ *   - a member is READY when b200_warp_poll reports it READABLE, or when it has a pending write (partial_write) and
+ *     credit for at least one frame.  The second rule is narrower than the Poller's WRITABLE (partial_write alone),
+ *     which would hand a blocked sender back to an edge-triggered consumer again and again;
+ *   - one consumer warp per set: take, drive the ends with the device calls, then b200_warp_ready_rearm each end it
+ *     has finished with.
+ * b200_ready_set_create: 1 <= capacity <= 8192 members; the queue and its control words live in device memory.  NULL
+ * and b200_last_error on failure.
+ * b200_ready_set_device fills the 64-byte handle the consumer kernel takes (0 / -1).
+ * b200_ready_set_destroy: the caller guarantees that no kernel uses the set.  -1 while the set has members.
+ * b200_ready_set_add: p must be device-owned, on the loopback wire and in no set.  A one-thread library kernel on the
+ * runtime's stream writes the member's note and queues one initial entry with the member disarmed, so a frame or a
+ * close that came before the add is not lost.  It may run while a consumer kernel takes from the set (a running
+ * server gets a new connection).  -1 and b200_last_error: p not claimed, p on the CUDA-IPC wire (its peer's kernels
+ * run in another process and cannot reach this queue), p already a member, the set full, or the queue could overflow
+ * because of stale entries (entries queued plus members reach the queue's size, twice the capacity rounded up to a
+ * power of two).
+ * Membership ends with the claim: b200_pair_device_release (and with it b200_pair_disconnect, b200_pair_init and
+ * b200_pool_putback) clears the member's note before it republishes.  The kernels that use the pair's handle must have
+ * finished before the release, as always; ops of the peer must not run across it.  Once the release returns nothing
+ * more is queued for the end, but an entry already queued can still be taken once, and counts against the queue's
+ * size until then.
+ */
+typedef struct b200_ready_set b200_ready_set;
+typedef struct b200_dev_ready_set {
+  void* queue;        /* control words, then the entries (device memory) */
+  uint32_t capacity;  /* members at most */
+  uint32_t size;      /* entries of the queue */
+  uint64_t _reserved[6];
+} b200_dev_ready_set;  /* POD, 64 bytes: pass it by pointer (device or pinned memory) or by value */
+b200_ready_set* b200_ready_set_create(uint32_t capacity);
+int b200_ready_set_device(b200_ready_set* s, b200_dev_ready_set* out);
+int b200_ready_set_destroy(b200_ready_set* s);
+int b200_ready_set_add(b200_ready_set* s, b200_pair* p, uint32_t key);
+
 #if defined(__cplusplus)
 static_assert(sizeof(b200_dev_pair) == 64, "b200_dev_pair is 64 bytes");
+static_assert(sizeof(b200_dev_ready_set) == 64, "b200_dev_ready_set is 64 bytes");
 #endif
 
 /* ------------------------------------------------------------------ poller */
