@@ -300,9 +300,10 @@ class Pair:
 
 
 class ReadySet:
-    """A device ready set (b200_ready_set_*): the queue a consumer kernel takes ready members' keys from
-    (include/b200_device.cuh: b200_warp_ready_take / b200_warp_ready_rearm).  Members are claimed Pairs on the loopback
-    wire; membership ends with the claim."""
+    """A device ready set (b200_ready_set_*): the queue consumer warps take ready members' keys from
+    (include/b200_device.cuh: b200_warp_ready_take / b200_warp_ready_rearm).  Any number of warps, in one kernel or
+    in several, may take from one set; each entry goes to one warp, which holds that member until its rearm returns 0.
+    Members are claimed Pairs on the loopback wire; membership ends with the claim."""
 
     def __init__(self, capacity):
         self.L = lib()

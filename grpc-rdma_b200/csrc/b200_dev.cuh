@@ -130,10 +130,10 @@ struct __align__(16) PairSeq {
 B200_HD PairSeq* pair_seq(PairDev* table, int slot) { return reinterpret_cast<PairSeq*>(table + kMaxPairs) + slot; }
 
 // ---- device ready sets (b200_ready_set_*, DESIGN.md §13 "Ready sets").  A set is a queue of 32-bit member keys in
-// device memory with one consumer warp; the paths that change a member's readiness append its key (notify_peer).
-// Control words: the consumer's head and the producers' tail on separate lines, then the entries.
+// device memory taken by any number of consumer warps; the paths that change a member's readiness append its key
+// (notify_peer).  Control words: the consumers' head and the producers' tail on separate lines, then the entries.
 struct __align__(128) ReadyQueue {
-  uint32_t head;  // next position the consumer takes (written by the consumer only)
+  uint32_t head;  // next position a consumer takes (advanced by the consumers' atomicCAS in ready_take)
   uint32_t _h[31];
   uint32_t tail;  // next position a producer claims (atomicAdd)
   uint32_t _t[31];

@@ -715,7 +715,7 @@ __device__ inline int warp_disconnect(PairDev* table, int slot, uint32_t lane) {
   return 1;
 }
 
-// ======================================================================= ready sets: the consumer (one warp per set)
+// ======================================================================= ready sets: the consumers (any number of warps)
 
 // A member is ready when poll_events reports READABLE, or when it has a pending write and credit for at least one
 // frame: the inverse of the host's "this Send cannot accept a byte" rule.  (The Poller's level-triggered WRITABLE on
@@ -733,34 +733,54 @@ __device__ __forceinline__ uint32_t ready_events(PairDev* table, int slot) {
 }
 
 // Up to `max` keys from the head of the queue into keys[]; stops at the first position whose entry has not been
-// stored yet.  Returns how many, every lane.
-__device__ inline uint32_t ready_take(ReadyQueue* q, uint32_t* keys, uint32_t max, uint32_t lane) {
-  const uint32_t head = VL(q->head), mask = VL(q->mask);
-  uint32_t n = 0;
-  while (n < max) {
-    const uint32_t i = n + lane;
-    bool ok = false;
-    uint64_t e = 0;
-    if (i < max) {
-      const uint32_t pos = head + i;
-      asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(e) : "l"(ready_entries(q) + (pos & mask)) : "memory");
-      ok = ready_entry_at(e, pos);
+// stored yet.  Returns how many, every lane; keys[] beyond that count are unspecified.  Any number of consumer warps
+// may take from one queue at once: the run [h, h + n) read from head h becomes this warp's by atomicCAS(head, h,
+// h + n), and a lost CAS (another consumer took first) reads again from the new head.  An empty run costs no atomic.
+// A won CAS returns the right keys: an entry is accepted only when its tag names its position, a slot is rewritten
+// only for position p + size, and b200_ready_set_add keeps entries queued plus members below size, so while head ==
+// h no producer holds a position at or beyond h + size; a CAS from h that wins saw head still at h.  (head is a
+// 32-bit counter: an ABA needs 2^32 taken entries between one warp's load and its CAS.)  A ticket atomicAdd(head)
+// would instead own positions whose producer may not have stored the entry yet, and the take would have to wait.
+// `retries` (may be null): lane 0 adds the lost CASes.
+__device__ inline uint32_t ready_take(ReadyQueue* q, uint32_t* keys, uint32_t max, uint32_t lane,
+                                      uint32_t* retries = nullptr) {
+  const uint32_t mask = VL(q->mask);
+  for (;;) {
+    uint32_t head = 0;
+    if (lane == 0) head = VL(q->head);
+    head = __shfl_sync(0xffffffffu, head, 0);
+    uint32_t n = 0;
+    while (n < max) {
+      const uint32_t i = n + lane;
+      bool ok = false;
+      uint64_t e = 0;
+      if (i < max) {
+        const uint32_t pos = head + i;
+        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(e) : "l"(ready_entries(q) + (pos & mask)) : "memory");
+        ok = ready_entry_at(e, pos);
+      }
+      const unsigned bad = __ballot_sync(0xffffffffu, !ok);
+      const uint32_t run = bad ? __ffs(bad) - 1 : 32;
+      if (lane < run) keys[i] = (uint32_t)e;
+      n += run;
+      if (run < 32) break;
     }
-    const unsigned bad = __ballot_sync(0xffffffffu, !ok);
-    const uint32_t run = bad ? __ffs(bad) - 1 : 32;
-    if (lane < run) keys[i] = (uint32_t)e;
-    n += run;
-    if (run < 32) break;
+    if (n == 0) return 0;
+    uint32_t won = 0;
+    if (lane == 0) {
+      won = atomicCAS(&q->head, head, head + n) == head;
+      if (!won && retries) (*retries)++;
+    }
+    __syncwarp();
+    if (__shfl_sync(0xffffffffu, won, 0)) return n;
   }
-  __syncwarp();
-  if (lane == 0 && n) VL(q->head) = head + n;
-  __syncwarp();
-  return n;
 }
 
 // The consumer is done with member `slot` of `q`: armed = 1, a fence, then the probe.  Ready and the exchange won:
 // the member's events (the consumer keeps it, nothing is queued).  Otherwise 0: a producer that saw armed == 1 has
 // queued the key, or nothing is pending and the next change will.  0 as well for an end that is not a member of `q`.
+// Once armed = 1 is stored, another consumer warp may take the member's new entry while this probe still runs: the
+// probe (poll_events, free_size) only reads, so the new holder's calls never run beside a write of this warp's.
 __device__ inline uint32_t ready_rearm(ReadyQueue* q, PairDev* table, int slot, uint32_t lane) {
   uint32_t ev = 0;
   if (lane == 0) {

@@ -124,10 +124,13 @@ __device__ inline int b200_warp_disconnect(const b200_dev_pair* h) {
 /* ---- ready sets: the device's epoll (b200_pair.h, DESIGN.md §13 "Ready sets") -------------------------------------
  *
  * A server warp that holds many claimed ends takes the keys of the ends whose readiness changed instead of scanning
- * them all.  ONE consumer warp per set; neither call waits.
- *   b200_warp_ready_take(s, keys, max): pops up to max keys into keys[] (device or pinned memory) and returns how many.
- *     They are hints: the consumer drives those ends with the calls above (Recv until it returns 0, Send, Disconnect).
- *     A taken key's frame, credit or close is visible to those calls.
+ * them all.  Any number of consumer warps may share one set (one CTA or many, one kernel or several); neither call
+ * waits.
+ *   b200_warp_ready_take(s, keys, max): pops up to max keys into keys[] (device or pinned memory) and returns how many;
+ *     keys[] beyond that count are unspecified.  Each entry goes to exactly one warp: the warp claims the run it read
+ *     with one atomicCAS on the queue's head and reads again when another warp took first.  An empty take does no
+ *     atomic.  The keys are hints: the consumer drives those ends with the calls above (Recv until it returns 0,
+ *     Send, Disconnect).  A taken key's frame, credit or close is visible to those calls.
  *   b200_warp_ready_rearm(s, h): the consumer has finished with member h for now.  It stores armed = 1, fences and
  *     probes.  When the end is READY (b200_warp_poll reports READABLE, or a write is pending and there is credit for
  *     one frame) and the call wins the end back from the producers, it returns the end's B200_EV_* bits: the consumer
@@ -136,6 +139,15 @@ __device__ inline int b200_warp_disconnect(const b200_dev_pair* h) {
  *     (no lost wakeup), and a member never has two entries queued.
  * The first entry of a member is queued by b200_ready_set_add, with the member disarmed: take it, serve, rearm.  An
  * entry of a released member can still be taken once; its key then names an end that is no longer a member.
+ * The holder rule, for consumers that share a set: a warp holds member m from the take that returned m's key, or from
+ * its rearm of m that returned non-zero, until its rearm of m returns 0 or it disconnects m.  Only the holder drives m
+ * (Recv, Send, Disconnect) and rearms it.  A member has at most one entry queued, and that entry is queued only after
+ * the holder's rearm stored armed = 1, so no two warps hold a member at once and the ops-in-flight rule holds with no
+ * lock in user code.  The new holder may take the entry while the old holder's rearm still probes; that probe only
+ * reads.  A warp that shares its set runs __threadfence() before each rearm: the rearm's own fence follows its store
+ * of armed = 1, and the next holder must see the cursors this warp's calls wrote and the warp's own per-member state.
+ * (With one consumer warp per set the fence is not needed.)  A warp may take up to max keys, but the members it holds
+ * are served by no other warp: take what the warp will serve soon.
  */
 __device__ inline uint32_t b200_warp_ready_take(const b200_dev_ready_set* s, uint32_t* keys, uint32_t max) {
   return b200::ready_take(static_cast<b200::ReadyQueue*>(s->queue), keys, max, b200_lane_id());

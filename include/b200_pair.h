@@ -238,8 +238,9 @@ int b200_pair_device_owned(const b200_pair* p);
  *   - a member is READY when b200_warp_poll reports it READABLE, or when it has a pending write (partial_write) and
  *     credit for at least one frame.  The second rule is narrower than the Poller's WRITABLE (partial_write alone),
  *     which would hand a blocked sender back to an edge-triggered consumer again and again;
- *   - one consumer warp per set: take, drive the ends with the device calls, then b200_warp_ready_rearm each end it
- *     has finished with.
+ *   - any number of consumer warps per set, in one CTA or in many, in one kernel or in several: each takes, drives
+ *     the ends it took with the device calls, then b200_warp_ready_rearm each end it has finished with.  Each entry
+ *     goes to exactly one warp, which holds the member until its rearm returns 0 (b200_device.cuh: the holder rule).
  * b200_ready_set_create: 1 <= capacity <= 8192 members; the queue and its control words live in device memory.  NULL
  * and b200_last_error on failure.
  * b200_ready_set_device fills the 64-byte handle the consumer kernel takes (0 / -1).
