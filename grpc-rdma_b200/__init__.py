@@ -141,6 +141,10 @@ _SIGS = {
     "b200_ready_set_device": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_ready_set_destroy": (C.c_int, [C.c_void_p]),
     "b200_ready_set_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32]),
+    "b200_ready_set_park": (C.c_int, [C.c_void_p]),
+    "b200_ready_set_wakeup_fd": (C.c_int, [C.c_void_p]),
+    "b200_ready_set_consume_wakeup": (None, [C.c_void_p]),
+    "b200_ready_set_rings": (C.c_uint64, [C.c_void_p]),
 }
 
 _lib = None
@@ -303,7 +307,8 @@ class ReadySet:
     """A device ready set (b200_ready_set_*): the queue consumer warps take ready members' keys from
     (include/b200_device.cuh: b200_warp_ready_take / b200_warp_ready_rearm).  Any number of warps, in one kernel or
     in several, may take from one set; each entry goes to one warp, which holds that member until its rearm returns 0.
-    Members are claimed Pairs on the loopback wire; membership ends with the claim."""
+    Members are claimed Pairs on the loopback wire; membership ends with the claim.  A parked set (park(), or
+    b200_warp_ready_park in a kernel) rings its doorbell at the next entry; the Poller then kicks wakeup_fd()."""
 
     def __init__(self, capacity):
         self.L = lib()
@@ -322,6 +327,28 @@ class ReadySet:
         """make the claimed `pair` a member with `key`; raises with b200_last_error's reason when refused"""
         if self.L.b200_ready_set_add(self.h, pair.h, key) != 0:
             raise RuntimeError("b200_ready_set_add failed: " + last_error())
+
+    def park(self):
+        """park the set from the host (no consumer may be taking): 0 parked, the next entry queued rings the
+        doorbell; 1 entries are queued, launch a server; raises on failure"""
+        rc = self.L.b200_ready_set_park(self.h)
+        if rc < 0:
+            raise RuntimeError("b200_ready_set_park failed: " + last_error())
+        return rc
+
+    def wakeup_fd(self):
+        """the set's eventfd, kicked by the Poller when the doorbell rings (the first call registers the set)"""
+        fd = self.L.b200_ready_set_wakeup_fd(self.h)
+        if fd < 0:
+            raise RuntimeError("b200_ready_set_wakeup_fd failed: " + last_error())
+        return fd
+
+    def consume_wakeup(self):
+        self.L.b200_ready_set_consume_wakeup(self.h)
+
+    def rings(self):
+        """doorbell rings so far: one per park that a later entry answered"""
+        return self.L.b200_ready_set_rings(self.h)
 
     def destroy(self):
         """no kernel may use the set; raises while it has members"""

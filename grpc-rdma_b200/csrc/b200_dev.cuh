@@ -132,15 +132,24 @@ B200_HD PairSeq* pair_seq(PairDev* table, int slot) { return reinterpret_cast<Pa
 // ---- device ready sets (b200_ready_set_*, DESIGN.md §13 "Ready sets").  A set is a queue of 32-bit member keys in
 // device memory taken by any number of consumer warps; the paths that change a member's readiness append its key
 // (notify_peer).  Control words: the consumers' head and the producers' tail on separate lines, then the entries.
+// Parking (DESIGN.md §13 "Parking"): `tail` is the low half of the 64-bit word at offset 128, whose bit 63 is the
+// parked bit; producers claim positions with a 64-bit atomicAdd on that word (carries out of the low half stop at bit
+// 62), and the one that clears the bit rings the set's doorbell.
 struct __align__(128) ReadyQueue {
   uint32_t head;  // next position a consumer takes (advanced by the consumers' atomicCAS in ready_take)
   uint32_t _h[31];
-  uint32_t tail;  // next position a producer claims (atomicAdd)
-  uint32_t _t[31];
+  uint32_t tail;     // next position a producer claims (low half of the 64-bit atomicAdd of ready_push)
+  uint32_t tail_hi;  // carries of tail in bits 0..30, the parked bit in bit 31 (bit 63 of the word)
+  uint64_t rings;    // doorbell rings so far (device count; each ring stores the new count into *bell)
+  uint32_t _t[28];
   uint32_t mask;  // entries - 1, set at creation
-  uint32_t _m[31];
+  uint32_t _m0;
+  uint64_t* bell;  // pinned, mapped host counter of the rings (b200_ready_set_rings), set at creation
+  uint32_t _m[28];
 };
 static_assert(sizeof(ReadyQueue) == 384, "ReadyQueue: three 128-byte lines");
+constexpr uint64_t kReadyParked = 1ull << 63;
+B200_HD unsigned long long* ready_tail_word(ReadyQueue* q) { return reinterpret_cast<unsigned long long*>(&q->tail); }
 // An entry is one 8-byte word: the key, and position + 1 in the top half (0: never written), so the consumer tells a
 // written entry from a slot whose producer has claimed it but not yet stored into it.
 B200_HD uint64_t* ready_entries(ReadyQueue* q) { return reinterpret_cast<uint64_t*>(q + 1); }
@@ -324,10 +333,12 @@ int cluster_capacity(int kind, int cluster);
 void launch_poll_scan(PairDev* pairs, const int32_t* slots, uint32_t* events, uint32_t* ready_count,
                       int32_t* ready_slots, int n, void* stream);
 // ready sets: load the library's kernels (before a user's consumer kernel may be resident); one-thread kernels that
-// make pair `slot` a member of `q` with `key`, and that run notify_peer for pair `slot` (b200_pair_disconnect)
+// make pair `slot` a member of `q` with `key`, that run notify_peer for pair `slot` (b200_pair_disconnect), and that
+// park `q` and write the park's result to *out (b200_ready_set_park)
 void load_kernels();
 void launch_ready_add(PairDev* pairs, int slot, ReadyQueue* q, uint32_t key, void* stream);
 void launch_ready_notify(PairDev* pairs, int slot, void* stream);
+void launch_ready_park(ReadyQueue* q, int* out, void* stream);
 
 // owners / pool / poller on three streams; returns false when the resident grids cannot be co-resident
 bool launch_service(const SvcParams& sp, void* s_owner, void* s_big, void* s_poll);

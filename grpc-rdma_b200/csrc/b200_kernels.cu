@@ -27,6 +27,7 @@
 #include <mutex>
 
 #include "b200_dev.cuh"
+#define B200_NOTIFY_OUT_OF_LINE 1  // notify_member is a call here (b200_warp.cuh)
 #include "b200_warp.cuh"  // memory helpers, readiness + mirrors, warp movers (shared with include/b200_device.cuh)
 #include "b200_block.cuh"  // the CTA pipeline: send_body / recv_body (shared with include/b200_device_block.cuh)
 
@@ -1050,6 +1051,8 @@ __global__ void k_ready_add(PairDev* pairs, int slot, ReadyQueue* q, uint32_t ke
   ready_push(q, key);
 }
 __global__ void k_ready_notify(PairDev* pairs, int slot) { notify_peer(pairs, slot); }
+// k_ready_park: b200_ready_set_park, the consumer's park run by one thread
+__global__ void k_ready_park(ReadyQueue* q, volatile int* out) { *out = (int)ready_park_one(q); }
 
 static void ensure_kernel_attrs() {
   static std::once_flag once;
@@ -1081,6 +1084,7 @@ static void ensure_kernel_attrs() {
   cudaFuncGetAttributes(&fa, k_cluster_recv);
   cudaFuncGetAttributes(&fa, k_ready_add);
   cudaFuncGetAttributes(&fa, k_ready_notify);
+  cudaFuncGetAttributes(&fa, k_ready_park);
   });
 }
 
@@ -1093,6 +1097,10 @@ void launch_ready_add(PairDev* pairs, int slot, ReadyQueue* q, uint32_t key, voi
 void launch_ready_notify(PairDev* pairs, int slot, void* stream) {
   ensure_kernel_attrs();
   k_ready_notify<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(pairs, slot);
+}
+void launch_ready_park(ReadyQueue* q, int* out, void* stream) {
+  ensure_kernel_attrs();
+  k_ready_park<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(q, out);
 }
 
 int svc_trace_read(unsigned long long* out16) {

@@ -272,18 +272,40 @@ __device__ __forceinline__ void publish_mirror_locked(PairDev* table, int slot) 
 // the consumer's store / fence / probe in b200_warp_ready_rearm, Dekker's pattern), then whoever takes `armed` from 1
 // to 0 appends the key, so a member has at most one entry queued.  The entry is stored with release semantics after
 // the change, and the consumer loads it with acquire semantics.
+// Parking (DESIGN.md §13 "Parking"): the position is claimed by a 64-bit atomicAdd on the word whose low half is
+// `tail`; when the value it returns has the parked bit, the producer clears the bit, and the one whose atomicAnd still
+// saw it rings the doorbell after its entry is stored: one ring per park.
+__device__ __forceinline__ void ready_ring(ReadyQueue* q) {
+  if ((atomicAnd(ready_tail_word(q), ~kReadyParked) & kReadyParked) == 0) return;  // another producer rang
+  const unsigned long long n = atomicAdd(reinterpret_cast<unsigned long long*>(&q->rings), 1ull) + 1ull;
+  uint64_t* bell = VL(q->bell);
+  __threadfence_system();  // the entry, and the change before it, reach the host's view before the count moves
+  asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(bell), "l"(n) : "memory");
+}
 __device__ __forceinline__ void ready_push(ReadyQueue* q, uint32_t key) {
-  const uint32_t pos = atomicAdd(&q->tail, 1u);
+  const unsigned long long w = atomicAdd(ready_tail_word(q), 1ull);
+  const uint32_t pos = (uint32_t)w;
   uint64_t* e = ready_entries(q) + (pos & VL(q->mask));
   asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(e), "l"(ready_entry(key, pos)) : "memory");
+  if (w & kReadyParked) ready_ring(q);
+}
+// The member's half is inlined into user kernels and called out of line by the library's kernels (b200_kernels.cu
+// defines B200_NOTIFY_OUT_OF_LINE).  Inlined with its ring path it made k_recv and k_svc_big spill; as a call it made
+// the device-call test kernels spill.  Either way, no kernel changes its registers, stack or spills.
+#ifdef B200_NOTIFY_OUT_OF_LINE
+static __device__ __noinline__ void notify_member(ReadyNote* n, ReadyQueue* q) {
+#else
+__device__ __forceinline__ void notify_member(ReadyNote* n, ReadyQueue* q) {
+#endif
+  __threadfence();
+  if (atomicExch(&n->armed, 0u) == 1u) ready_push(q, VL(n->key));
 }
 __device__ __forceinline__ void notify_peer(PairDev* table, int peer_slot) {
   if (peer_slot < 0) return;
   ReadyNote* n = ready_note(table, peer_slot);
   ReadyQueue* q = VL(n->set);
   if (q == nullptr) return;
-  __threadfence();
-  if (atomicExch(&n->armed, 0u) == 1u) ready_push(q, VL(n->key));
+  notify_member(n, q);
 }
 
 // ======================================================================= one call by one warp, any size
@@ -793,6 +815,22 @@ __device__ inline uint32_t ready_rearm(ReadyQueue* q, PairDev* table, int slot, 
     }
   }
   return __shfl_sync(0xffffffffu, ev, 0);
+}
+
+// Park the set (DESIGN.md §13 "Parking"), by the one warp that still takes from it, holding no member: set the parked
+// bit, and compare the tail it covered with head.  Equal: 0, the set is parked and the next push rings.  Not equal:
+// entries are queued, so clear the bit again; if it was still set no producer rang, and the caller has work (1).  If a
+// producer cleared it first, its ring is on its way and the set counts as parked (0).  Park and push are
+// read-modify-writes of one word, so their order is that word's coherence order: no fence is needed.
+// ready_park_one is the park by one thread (k_ready_park runs it for b200_ready_set_park).
+__device__ inline uint32_t ready_park_one(ReadyQueue* q) {
+  const unsigned long long w = atomicOr(ready_tail_word(q), kReadyParked);
+  if ((uint32_t)w == VL(q->head)) return 0;
+  return (atomicAnd(ready_tail_word(q), ~kReadyParked) & kReadyParked) ? 1u : 0u;
+}
+__device__ inline uint32_t ready_park(ReadyQueue* q, uint32_t lane) {
+  const uint32_t busy = lane == 0 ? ready_park_one(q) : 0u;
+  return __shfl_sync(0xffffffffu, busy, 0);
 }
 
 }  // namespace b200

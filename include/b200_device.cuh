@@ -157,4 +157,24 @@ __device__ inline uint32_t b200_warp_ready_rearm(const b200_dev_ready_set* s, co
                            h->slot, b200_lane_id());
 }
 
+/* b200_warp_ready_park(s): park the set so that the server may exit, warp-collective (b200_pair.h and DESIGN.md §13
+ * "Parking").  The next entry queued on a parked set rings its doorbell once, and the Poller kicks the set's eventfd.
+ * The rule:
+ *   - one warp calls it, once no other consumer warp of the set will take again;
+ *   - that warp holds no member: each of its rearms returned 0, or it disconnected the member;
+ *   - 0: the set is parked (or a ring is already on its way), and the kernel may exit;
+ *   - non-zero: entries are queued and nothing rang; the warp must take and serve again (and park again later).  With
+ *     many warps the last one to go idle may serve alone.
+ * The multi-warp exit (tests/native/device_ready_park.cu): each warp counts empty takes, and after K in a row it adds
+ * one to an idle counter in device memory and stops taking.  The warp whose atomicAdd returns warps - 1 is the last:
+ * it parks; while the park returns non-zero it takes, serves and rearms alone, then parks again.  The kernel exits
+ * when that park returns 0.
+ *
+ *   if (atomicAdd(&idle, 1) == warps - 1)           // lane 0, broadcast to the warp
+ *     while (b200_warp_ready_park(s)) serve_until_empty(s);
+ */
+__device__ inline uint32_t b200_warp_ready_park(const b200_dev_ready_set* s) {
+  return b200::ready_park(static_cast<b200::ReadyQueue*>(s->queue), b200_lane_id());
+}
+
 #endif /* B200_DEVICE_CUH */

@@ -257,6 +257,22 @@ int b200_pair_device_owned(const b200_pair* p);
  * finished before the release, as always; ops of the peer must not run across it.  Once the release returns nothing
  * more is queued for the end, but an entry already queued can still be taken once, and counts against the queue's
  * size until then.
+ *
+ * Parking (DESIGN.md §13 "Parking"): a server kernel need not stay resident while its set is idle.  It parks the set
+ * (b200_warp_ready_park) and exits; the next entry queued on a parked set -- a frame, credit or close of a member, or
+ * b200_ready_set_add's initial entry -- rings the set's doorbell once: a 64-bit counter in pinned host memory.  The
+ * Poller threads turn a doorbell that moved into a kick of the set's eventfd; the application polls that fd and
+ * launches the server again.  A release of a member rings nothing.
+ * b200_ready_set_park: the same park from the host, through a one-thread library kernel on the runtime's stream: 0 the
+ * set is parked, 1 entries are queued (launch a server; the set is not parked), -1 and b200_last_error on failure.  No
+ * consumer may take from the set while it runs.  A set starts unparked; parking it before any server runs launches
+ * servers on demand, and parking it after the host stopped its server itself makes the next change ring.  The kernel is
+ * loaded with the library's others, so a host park may run beside resident kernels.
+ * b200_ready_set_wakeup_fd: the set's eventfd (-1 on failure).  The first call creates it, registers the set with the
+ * Poller and starts the Poller's threads, as b200_poller_add does; a ring from before the call signals it as well.
+ * b200_ready_set_consume_wakeup: reads the eventfd back to not-readable.
+ * b200_ready_set_rings: the doorbell, the rings so far; a wait-free read of pinned memory, for a host that busy-polls
+ * for a while before it waits on the fd.  b200_ready_set_destroy unregisters the set and closes its fd.
  */
 typedef struct b200_ready_set b200_ready_set;
 typedef struct b200_dev_ready_set {
@@ -269,6 +285,10 @@ b200_ready_set* b200_ready_set_create(uint32_t capacity);
 int b200_ready_set_device(b200_ready_set* s, b200_dev_ready_set* out);
 int b200_ready_set_destroy(b200_ready_set* s);
 int b200_ready_set_add(b200_ready_set* s, b200_pair* p, uint32_t key);
+int b200_ready_set_park(b200_ready_set* s);
+int b200_ready_set_wakeup_fd(b200_ready_set* s);
+void b200_ready_set_consume_wakeup(b200_ready_set* s);
+uint64_t b200_ready_set_rings(const b200_ready_set* s);
 
 #if defined(__cplusplus)
 static_assert(sizeof(b200_dev_pair) == 64, "b200_dev_pair is 64 bytes");
